@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — benchmark of the B200-native kajiya ReSTIR-GI hot path (rtdgi + irradiance cache + rtr + taa).
+"""bench.py — benchmark of the H100-native kajiya ReSTIR-GI hot path (rtdgi + irradiance cache + rtr + taa).
 
-    python bench.py --gpus N --steps K --warmup W            # this implementation (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this implementation (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K ...  # the CPU restatement of the reference's path, all host threads
 
 A "step" is one frame of the hot path over one synthetic batch of G-buffer inputs.  The headline workload is the WHOLE path on the
@@ -23,6 +23,9 @@ with ms/frame as `ms_per_step`.
              sample of the same workload — replayed G-buffers, i.e. exactly the passes the GPU arm times.
 At N > 1 ONE frame is tile-sharded over the ranks (strong scaling); `parity` compares every rank's band with an untiled render of the
 same frames on that rank.
+`--dump-outputs DIR`: after the timed steps, the headline's result image of the last timed frame (what the host-buffer call hands its
+caller) is written as DIR/<image name>.npy in float32, so that two builds can be compared output for output; the inputs of a run depend
+only on its arguments.
 """
 import argparse, ctypes as C, hashlib, json, os, subprocess, sys, threading, time
 
@@ -97,7 +100,7 @@ def pass_bytes(label, F, Hh, O=None, validation_frame_fraction=1.0 / 3.0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     def __init__(self, gpu_index):
         self.samples, self.proc, self.gpu = [], None, gpu_index
@@ -142,7 +145,7 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def build_world(lib, workload, device=0, tile=None):
@@ -161,7 +164,7 @@ def config_of(workload):
     out = flags.get("upscale") or (W, H)
     return {"workload": workload, "baseline_config": BASELINE_CONFIG.get(workload), "scene": fn, "resolution": [W, H], "output_resolution": list(out),
             "spatial_reuse_passes": spatial, "features": sorted(k for k, v in flags.items() if v and k != "upscale"),
-            "inputs": "a ring of distinct jittered G-buffers larger than L2 (126 MB), replayed; e2e uploads them from pinned host memory"}
+            "inputs": "a ring of distinct jittered G-buffers larger than L2 (50 MB), replayed; e2e uploads them from pinned host memory"}
 
 
 def pinned_empty(torch, nbytes):
@@ -174,8 +177,9 @@ def result_image_name(workload):
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU arm
-def measure_frames(lib, torch, dist, workload, K, Wm, rank, world_size, local_rank, nslots, streaming=True):
-    """device-resident, per-pass and end-to-end legs of one frame workload; returns a dict on every rank (reduced over ranks)"""
+def measure_frames(lib, torch, dist, workload, K, Wm, rank, world_size, local_rank, nslots, streaming=True, dump=None):
+    """device-resident, per-pass and end-to-end legs of one frame workload; returns a dict on every rank (reduced over ranks).
+    `dump`: a dict that receives the result image of the last timed frame"""
     w, view, W, H = build_world(lib, workload, device=local_rank, tile=(rank, world_size) if world_size > 1 else None)
     if world_size > 1:
         uid = [None]
@@ -234,6 +238,8 @@ def measure_frames(lib, torch, dist, workload, K, Wm, rank, world_size, local_ra
     ms_total = w.timer_elapsed_ms(1000, 1001)
     barrier()
     st = w.stats()
+    if dump is not None:
+        dump[result_image_name(workload)] = w.image(result_image_name(workload))
     rays = st["closest_rays"] + st["any_hit_rays"]
     closest_share = st["closest_rays"] / max(rays, 1)
     launches = lib.dll.kjb_launch_count(w.ctx) - launches0
@@ -393,10 +399,10 @@ def summarize(m, world_size, peak, ncu_table):
             "frame": {"algorithmic_bytes": frame_bytes, "achieved_gbs": frame_bytes / (frame_ms * 1e-3) / 1e9, "frac": frame_bytes / (frame_ms * 1e-3) / 1e9 / (peak * world_size)},
             "per_pass_ms": {k: round(v, 5) for k, v in sorted(per_pass.items(), key=lambda kv: -share[kv[0]])}}
     if tab and tab.get("warp_inst"):
-        # these kernels are bound by instruction issue, not DRAM: also report the dominant kernel against 148 SMs x 4 schedulers x SM clock
-        sm_mhz = 1965.0
+        # these kernels are bound by instruction issue, not DRAM: also report the dominant kernel against 132 SMs x 4 schedulers x SM clock
+        sm_mhz = 1980.0
         ach = tab["warp_inst"] / (per_pass[dom] * 1e-3) / 1e9
-        roof["issue_slots"] = {"warp_inst_per_launch": tab["warp_inst"], "achieved_ginst_s": ach, "peak_ginst_s": 148 * 4 * sm_mhz * 1e-3, "frac": ach / (148 * 4 * sm_mhz * 1e-3), "source": tab.get("source")}
+        roof["issue_slots"] = {"warp_inst_per_launch": tab["warp_inst"], "achieved_ginst_s": ach, "peak_ginst_s": 132 * 4 * sm_mhz * 1e-3, "frac": ach / (132 * 4 * sm_mhz * 1e-3), "source": tab.get("source")}
     return {"ms_per_step": frame_ms, "value": m["rays"] / (m["ms_total"] * 1e-3), "unit": "rays/s", "rays_per_frame": m["rays"] / K,
             "ray_kinds": {"closest_hit_per_frame": m["rays"] / K * m.get("closest_share", 0.0), "any_hit_per_frame": m["rays"] / K * (1.0 - m.get("closest_share", 0.0)),
                           "note": "closest-hit rays carry shading (material fetch, sun shadow ray, cache lookup); any-hit rays are visibility only"},
@@ -474,6 +480,8 @@ def run_cuda(args):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     torch.cuda.set_device(local_rank)
     lib = kajiya_b200.lib()   # raises without the CUDA extension: no fallback
+    if args.dump_outputs and world_size > 1:   # a rank of a tile-sharded frame holds only its band of the result
+        raise SystemExit("--dump-outputs: the result image is written by single-GPU runs only")
     K, Wm = args.steps, args.warmup
     peak, peak_src = load_peaks()
     ncu_table = load_ncu_table()
@@ -485,9 +493,9 @@ def run_cuda(args):
     else:
         names = [headline]
     clocks = ClockSampler(local_rank); clocks.start()
-    windows, entries, head = [], [], None
+    windows, entries, head, dump = [], [], None, {}
     for name in names:
-        Kc = K if name == headline else max(4, min(K, 16))   # secondary configurations: a shorter timed region keeps the default run within minutes
+        Kc = K if name == headline else min(K, 16)   # secondary configurations: a shorter timed region keeps the default run within minutes
         Wc = Wm if name == headline else max(3, min(Wm, 4))
         if name == "cornell_256_reference_pt":
             if rank == 0:
@@ -500,7 +508,8 @@ def run_cuda(args):
             if dist is not None:
                 dist.barrier()
             continue
-        m = measure_frames(lib, torch, dist, name, Kc, Wc, rank, world_size, local_rank, nslots=16 if name == headline else 6, streaming=not args.no_streaming)
+        m = measure_frames(lib, torch, dist, name, Kc, Wc, rank, world_size, local_rank, nslots=16 if name == headline else 6, streaming=not args.no_streaming,
+                           dump=dump if args.dump_outputs and name == headline else None)
         windows += m["windows"]
         par = None
         if world_size > 1:
@@ -517,7 +526,7 @@ def run_cuda(args):
                                   f"(the ranks actually traced {m['rays_traced_all_ranks'] / Kc:.0f} per frame including halo recompute)")
                 e["parity"] = par
             if world_size == 1 and name in (headline, "cornell_1080p_rtdgi_1s1t") and not args.no_fast_math:
-                e["fast_math"] = measure_fast_math(torch, name, max(4, min(Kc, 16)), Wc, local_rank)
+                e["fast_math"] = measure_fast_math(torch, name, min(Kc, 16), Wc, local_rank)
                 if "ms_per_step" in e["fast_math"]:
                     e["fast_math"]["exact_over_fast"] = e["ms_per_step"] / e["fast_math"]["ms_per_step"]
             if world_size == 1 and not args.no_cpu_baseline:
@@ -526,6 +535,8 @@ def run_cuda(args):
             if name == headline:
                 head = e
     clock_info = clocks.stop(windows)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, dump)
     if rank != 0:
         if dist is not None:
             dist.destroy_process_group()
@@ -540,6 +551,22 @@ def run_cuda(args):
     print(json.dumps(out))
     if dist is not None:
         dist.destroy_process_group()
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, arrays):
+    """DIR/<name>.npy in float32, at most DUMP_BYTES in all: an array over its share is replaced by a fixed, seeded sample of its rows"""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    share = (DUMP_BYTES - 4096 * len(arrays)) // max(len(arrays), 1)   # 4 KiB per file for the .npy header
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float32)
+        if a.nbytes > share:
+            rows = np.random.default_rng(0).choice(a.shape[0], share // (a.nbytes // a.shape[0]), replace=False)
+            a = a[np.sort(rows)]
+        np.save(os.path.join(dirname, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------------------------- CPU arms
@@ -633,7 +660,7 @@ def run_reference(args):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=32)
+    ap.add_argument("--steps", type=int, default=32, help="timed frames of the headline; the secondary configurations and the fast-math leg time min(steps, 16)")
     ap.add_argument("--warmup", type=int, default=6)
     ap.add_argument("--impl", default="kajiya_b200", choices=["kajiya_b200", "reference"])
     ap.add_argument("--workload", default=HEADLINE, choices=sorted(WORKLOADS), help="the headline workload of the line")
@@ -642,6 +669,7 @@ def main():
     ap.add_argument("--no-fast-math", action="store_true", help="skip the libkjb_fast.so leg (the price of the exact numeric contract)")
     ap.add_argument("--no-streaming", action="store_true", help="e2e leg with the blocking call (upload, passes, download serialised)")
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the headline's result image of the last timed frame to DIR/<name>.npy (float32); one GPU only")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":

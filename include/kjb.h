@@ -1,4 +1,4 @@
-/* kjb.h — C-ABI of the B200-native kajiya ReSTIR-GI hot path.
+/* kjb.h — C-ABI of the H100-native kajiya ReSTIR-GI hot path.
  *
  * kajiya has no FFI: its extension point is the Rust closure handed to
  * `PassBuilder::render` (crates/lib/kajiya-rg/src/pass_builder.rs:325-337), normally built
@@ -160,7 +160,7 @@ int  kjb_create(int device, kjb_context **out_ctx);
 void kjb_destroy(kjb_context *ctx);
 int  kjb_sync(kjb_context *ctx);
 const char *kjb_last_error(kjb_context *ctx);
-/* which implementation is behind the pointer: "cuda-sm100a", "emu-cpu", "oracle-cpu" */
+/* which implementation is behind the pointer: "cuda-sm90a", "emu-cpu", "oracle-cpu" */
 const char *kjb_backend_name(void);
 /* number of device kernels launched through this context so far (0 for the oracle) */
 uint64_t kjb_launch_count(kjb_context *ctx);
@@ -253,6 +253,12 @@ int  kjb_event_synchronize(kjb_context *ctx, uint32_t event);                   
  * "restir temporal", kjb_image_upload/clear/copy/fill, kjb_set_frame_constants); a host that writes those two images by other means
  * (interop) must leave the option off. */
 #define KJB_OPTION_HALF_RES_POSITION_CACHE 1u
+/* KJB_OPTION_ORDERED_CACHE_SCHEDULE (default 1 in the CUDA build, 0 in the CPU emulator): how the parallel kernels that touch the irradiance
+ * cache resolve their conflicts.  1 = decisions that do not depend on the order the threads run in, so the same inputs give the same
+ * frames on every run (claimed cells get entries at the next cache chain, votes go to the smallest hash; kjb_ircache.cuh).  0 = the
+ * reference's atomics as they land (scheduling dependent on the GPU; in launch order, like the oracle, in the emulator).  Set it before the
+ * first frame with the cache: it cannot change once the ordered schedule holds pending claims. */
+#define KJB_OPTION_ORDERED_CACHE_SCHEDULE 2u
 int  kjb_set_option(kjb_context *ctx, uint32_t option, uint32_t value);
 /* CUDA Graph replay of a frame's passes (the reference records one command buffer per frame, graph.rs:865-867; ~40 kernel launches here):
  * every pass enqueued on the compute queue between the two calls is RECORDED instead of launched; kjb_graph_end turns the recording into
@@ -273,8 +279,9 @@ int  kjb_set_pass_queue(kjb_context *ctx, uint32_t queue);
 int  kjb_async_passes_supported(kjb_context *ctx);
 int  kjb_graph_stats(kjb_context *ctx, uint64_t out_launches_instantiations[2]);
 int  kjb_set_scissor(kjb_context *ctx, uint32_t y0, uint32_t y1);
-/* Determinism aid: while on, every pass that touches the (racy by design) irradiance cache runs on ONE device thread in the launch
- * order of its parallel kernel. Orders of magnitude slower; for reproducing cache states and for bit-exact parity tests. */
+/* Oracle schedule: while on, every pass that touches the irradiance cache runs on ONE device thread in the launch order of its
+ * parallel kernel, with the reference's atomics — the oracle's schedule. Orders of magnitude slower; for bit-exact parity tests.
+ * Like KJB_OPTION_ORDERED_CACHE_SCHEDULE, switch it on before the first frame with the cache. */
 int  kjb_set_debug_serial(kjb_context *ctx, uint32_t on);
 
 /* ------------------------------------------------------------------ input producers (SURVEY §8f N1/N2, needed to feed the path) */

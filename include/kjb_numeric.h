@@ -118,7 +118,7 @@ KJB_HD float kjb_fma(float a, float b, float c) {
 /* HLSL/DXIL FMin/FMax = IEEE minNum/maxNum: a NaN operand loses (the shaders rely on it, e.g. `max(0.0, dot(n, NaN_dir))`
  * for neighbours at depth 0 in restir_resolve.hlsl:112-114).  Signed zeros are ordered -0 < +0 and two NaNs give the canonical
  * 0x7fffffff (IEEE 754-2019 minimumNumber / maximumNumber): exactly what the single FMNMX instruction behind fminf/fmaxf returns on
- * sm_100a (probed: tools/probe_minmax.cu, profiles/r01u_probe_minmax.txt), spelled out for the host. */
+ * sm_90a (probed: tools/probe_minmax.cu), spelled out for the host. */
 KJB_HD float kjb_min(float a, float b) {
 #if defined(__CUDA_ARCH__)
     return fminf(a, b);

@@ -1,4 +1,4 @@
-"""kajiya_b200 — B200-native (sm_100a CUDA) implementation of kajiya's ReSTIR-GI hot path.
+"""kajiya_b200 — H100-native (sm_90a CUDA) implementation of kajiya's ReSTIR-GI hot path.
 
 The package is a thin host-side mirror of the reference's renderer API over the C-ABI shared
 library `kajiya_b200/csrc/libkjb.so` (hand-written CUDA kernels + the C++ frame driver).
@@ -23,7 +23,7 @@ def lib():
             raise KjbError(f"CUDA extension missing: {LIB_PATH} (run `python -c 'import __graft_entry__ as g; g.build()'`). "
                            "kajiya_b200 has no CPU fallback.")
         _lib = KjbLib(LIB_PATH)
-        if _lib.backend != "cuda-sm100a":
+        if _lib.backend != "cuda-sm90a":
             raise KjbError(f"unexpected backend {_lib.backend!r} behind {LIB_PATH}")
     return _lib
 
@@ -41,6 +41,6 @@ def lib_fast():
         if not os.path.exists(FAST_LIB_PATH):
             raise KjbError(f"fast-math build missing: {FAST_LIB_PATH}")
         _fast = KjbLib(FAST_LIB_PATH)
-        if _fast.backend != "cuda-sm100a-fast":
+        if _fast.backend != "cuda-sm90a-fast":
             raise KjbError(f"unexpected backend {_fast.backend!r} behind {FAST_LIB_PATH}")
     return _fast

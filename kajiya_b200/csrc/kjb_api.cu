@@ -46,9 +46,9 @@ TileSource tile_source(kjb_context* c, const kjb_image& img, uint32_t box_w, uin
     return t;
 }
 int tile_mode(std::initializer_list<const TileSource*> sources) {
-    // Preference: per-row bulk copies (UBLKCP) by default.  The tensor-map form (UTMALDG) is complete but opt-in: on the B200 boxes of this
-    // pool every cp.async.bulk.tensor — ours, and NVIDIA's own libcu++ wrapper in tools/tma_probe.cu — raises "illegal instruction" while
-    // cp.async.bulk works (profiles/r02_tma_probe.txt), so it cannot be the default here.  KJB_TILE_MODE=loads is the A/B switch.
+    // Preference: per-row bulk copies (UBLKCP) by default.  The tensor-map form (UTMALDG, KJB_TILE_MODE=tensor) runs bit-exact on H100 too,
+    // at the same frame time within the run-to-run spread (DESIGN §5a), so the default stays with the form the whole GPU suite runs.
+    // KJB_TILE_MODE=loads is the A/B switch.
     static const int pref = [] {
         const char* e = getenv("KJB_TILE_MODE"); const char* off = getenv("KJB_NO_TMA");
         if (off && off[0] == '1') return KJB_TILE_LOADS;
@@ -146,9 +146,9 @@ int kjb_abi_version(void) { return KJB_ABI_VERSION; }
 const char* kjb_backend_name(void) { return "emu-cpu"; }
 #else
 #if defined(KJB_FAST)
-const char* kjb_backend_name(void) { return "cuda-sm100a-fast"; }   // approximate-math build (include/kjb_numeric.h, KJB_FAST): never the default
+const char* kjb_backend_name(void) { return "cuda-sm90a-fast"; }   // approximate-math build (include/kjb_numeric.h, KJB_FAST): never the default
 #else
-const char* kjb_backend_name(void) { return "cuda-sm100a"; }
+const char* kjb_backend_name(void) { return "cuda-sm90a"; }
 #endif
 #endif
 
@@ -181,6 +181,7 @@ void kjb_destroy(kjb_context* c) {
     dev_free(c->d_vertices); dev_free(c->d_meshes); dev_free(c->d_instances); dev_free(c->d_nodes); dev_free(c->d_tris); dev_free(c->d_tri_info);
     dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box); dev_free(c->d_tri_box);
     dev_free(c->d_tex_data); dev_free(c->d_tex_desc); dev_free(c->d_lights); dev_free(c->d_ray_counters); dev_free(c->d_prev_instances); dev_free(c->d_resolve_offsets);
+    for (auto& kv : c->ircache_scratch) { const auto& s = kv.second; dev_free(s.claim_rank); dev_free(s.claim_vertex); dev_free(s.life_pending); dev_free(s.scan); dev_free(s.claim_bits); dev_free(s.aux_prev); dev_free(s.entry_vertex); }
 #if !defined(KJB_EMU)
     if (c->pinned_staging) cudaFreeHost(c->pinned_staging);
     for (auto& ge : c->graph_execs) if (ge) cudaGraphExecDestroy(ge);
@@ -210,8 +211,17 @@ int kjb_image_alloc(kjb_context* c, uint32_t w, uint32_t h, uint32_t layers, uin
     out->data = dev_alloc(image_bytes(*out));   // zero-filled
     return out->data ? 0 : c->fail("kjb_image_alloc: out of device memory");
 }
+// the cache scratch of a freed life buffer goes with it: the address may be reused by a cache that must not inherit its pending claims
+static void drop_ircache_scratch(kjb_context* c, const void* p) {
+    auto it = c->ircache_scratch.find(p);
+    if (it == c->ircache_scratch.end()) return;
+    dev_sync(c);
+    const auto& s = it->second; dev_free(s.claim_rank); dev_free(s.claim_vertex); dev_free(s.life_pending); dev_free(s.scan); dev_free(s.claim_bits); dev_free(s.aux_prev); dev_free(s.entry_vertex);
+    c->ircache_scratch.erase(it);
+}
 int kjb_image_free(kjb_context* c, kjb_image* img) {
     for (auto it = c->tile_sources.begin(); it != c->tile_sources.end();) { if (std::get<0>(it->first) == img->data) it = c->tile_sources.erase(it); else ++it; }   // the address may be reused
+    drop_ircache_scratch(c, img->data);
     dev_free(img->data); img->data = nullptr; return 0;
 }
 int kjb_image_clear(kjb_context* c, const kjb_image* img) { c->invalidate_positions(); return dev_memset(c, img->data, 0, image_bytes(*img)); }
@@ -274,7 +284,7 @@ int kjb_event_synchronize(kjb_context* c, uint32_t e) {
 }
 #endif
 int kjb_buffer_alloc(kjb_context* c, uint64_t n, kjb_buffer* out) { out->data = dev_alloc(n); out->size_bytes = n; return out->data ? 0 : c->fail("kjb_buffer_alloc: out of device memory"); }
-int kjb_buffer_free(kjb_context*, kjb_buffer* b) { dev_free(b->data); b->data = nullptr; return 0; }
+int kjb_buffer_free(kjb_context* c, kjb_buffer* b) { drop_ircache_scratch(c, b->data); dev_free(b->data); b->data = nullptr; return 0; }
 int kjb_buffer_upload(kjb_context* c, const kjb_buffer* dst, uint64_t off, const void* src, uint64_t n) { return dev_h2d(c, (char*)dst->data + off, src, n); }
 int kjb_buffer_download(kjb_context* c, const kjb_buffer* src, uint64_t off, void* dst, uint64_t n) { return dev_d2h(c, dst, (const char*)src->data + off, n); }
 
@@ -451,9 +461,18 @@ int kjb_set_frame_constants(kjb_context* c, const kjb_frame_constants* fc, const
     return 0;
 }
 int kjb_set_scissor(kjb_context* c, uint32_t y0, uint32_t y1) { c->scissor_y0 = y0; c->scissor_y1 = y1; return 0; }
-int kjb_set_debug_serial(kjb_context* c, uint32_t on) { c->debug_serial = on != 0; return 0; }
+// the ordered cache schedule keeps claims pending until the next chain: another schedule would find cells flagged with no entry behind them
+static bool ordered_cache_has_run(const kjb_context* c) { return !c->ircache_scratch.empty(); }
+int kjb_set_debug_serial(kjb_context* c, uint32_t on) {
+    if (on && !c->debug_serial && ordered_cache_has_run(c)) return c->fail("kjb_set_debug_serial: the irradiance cache already runs on the ordered schedule; switch before its first frame");
+    c->debug_serial = on != 0; return 0;
+}
 int kjb_set_option(kjb_context* c, uint32_t option, uint32_t value) {
     if (option == KJB_OPTION_HALF_RES_POSITION_CACHE) { c->opt_position_cache = value != 0; c->invalidate_positions(); return 0; }
+    if (option == KJB_OPTION_ORDERED_CACHE_SCHEDULE) {
+        if (!value && c->ordered_cache && ordered_cache_has_run(c)) return c->fail("kjb_set_option: the irradiance cache already runs on the ordered schedule; switch before its first frame");
+        c->ordered_cache = value != 0; return 0;
+    }
     return c->fail("kjb_set_option: unknown option");
 }
 int kjb_set_luts(kjb_context* c, const kjb_image* fg, const kjb_image* bn) {

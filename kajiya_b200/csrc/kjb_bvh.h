@@ -1,9 +1,8 @@
-// Software acceleration structure for B200 (no RT cores, no Vulkan): a single flattened WORLD-SPACE BVH2.
+// Software acceleration structure for H100 (no RT cores, no Vulkan): a single flattened WORLD-SPACE BVH2.
 //
 // The reference keeps a two-level driver structure (BLAS per mesh + TLAS rebuilt per frame,
-// crates/lib/kajiya-backend/src/vulkan/ray_tracing.rs:96-260,455-520) because RT hardware wants it.  On B200 the
-// whole flattened scene (2 M triangles = 96 MB of triangles + 64 MB of nodes) fits the 126 MB L2 to a large part, so
-// one level wins: no per-instance ray transform, one traversal loop.  "rebuild tlas" re-flattens when transforms change.
+// crates/lib/kajiya-backend/src/vulkan/ray_tracing.rs:96-260,455-520) because RT hardware wants it.  Without
+// RT hardware, one level wins: no per-instance ray transform, one traversal loop.  "rebuild tlas" re-flattens when transforms change.
 //
 // Layout (Aila-Laine style, 64-byte nodes holding BOTH children's boxes => one 64 B line per traversal step):
 //   n0 = (c0.lo.x, c0.hi.x, c0.lo.y, c0.hi.y)   n1 = (c1.lo.x, c1.hi.x, c1.lo.y, c1.hi.y)

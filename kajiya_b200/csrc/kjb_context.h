@@ -1,5 +1,5 @@
 // Library context + the thin device-runtime layer the entry points use.
-// In the product this is the CUDA runtime on one stream of one B200.  When the translation unit is compiled by the
+// In the product this is the CUDA runtime on one stream of one H100.  When the translation unit is compiled by the
 // test-only CPU launch emulator (KJB_EMU, tests/emu/), the same six calls map to libc — that build is never shipped,
 // never loaded by kajiya_b200, and reports itself as "emu-cpu".
 #pragma once
@@ -66,6 +66,9 @@ struct kjb_context {
     kjb::Globals g;   // host copy, passed by value to every kernel
     // tensor maps of the images the tiled kernels stage through TMA, one per (image, box): built on first use, dropped when the image is freed
     std::map<std::tuple<const void*, uint32_t, uint32_t, uint32_t, uint32_t, uint32_t>, kjb::TileSource> tile_sources;
+    // device scratch of the irradiance cache's ordered schedule (kjb_ircache.cuh), one set per cache, keyed by its life_buf; freed with that buffer
+    struct IrcacheScratch { void* claim_rank; void* claim_vertex; void* life_pending; void* scan; void* claim_bits; void* aux_prev; void* entry_vertex; };
+    std::map<const void*, IrcacheScratch> ircache_scratch;
 
     // multi-GPU transport (tile-sharded frames)
     kjb_allgather_fn ag_fn = nullptr; void* ag_user = nullptr; uint32_t rank = 0, nranks = 1; void* nccl_comm = nullptr;
@@ -78,6 +81,11 @@ struct kjb_context {
     PosCache pos_a, pos_b; uint64_t epoch_a = 0, epoch_b = 0; bool opt_position_cache = false;
     void invalidate_positions() { epoch_a++; epoch_b++; }
     bool debug_serial = false;   // kjb_set_debug_serial: cache-touching passes run on one GPU thread in launch order
+#if defined(KJB_EMU)
+    bool ordered_cache = false;  // KJB_OPTION_ORDERED_CACHE_SCHEDULE: the emulator runs launches in order, like the oracle
+#else
+    bool ordered_cache = true;
+#endif
     kjb::Rows rows_for(uint32_t H) const {
         kjb::Rows r; r.y0 = 0; r.y1 = int(H);
         if (scissor_y1 > scissor_y0) { r.y0 = int(scissor_y0 < H ? scissor_y0 : H); r.y1 = int(scissor_y1 < H ? scissor_y1 : H); }

@@ -1,4 +1,4 @@
-// Device-side numeric core of the B200 kernels: HLSL-style vector math, RNG, packing, reservoirs,
+// Device-side numeric core of the H100 kernels: HLSL-style vector math, RNG, packing, reservoirs,
 // view/ray context, BRDFs, sun/atmosphere, typed image access.
 //
 // Re-derived from kajiya's shader includes (paths relative to /root/reference/assets/shaders/inc/):

@@ -3,9 +3,20 @@
 //
 // The cache is a racy structure BY DESIGN upstream (docs/gi-overview.md "Irradiance cache"; ircache.rs:68-76 binds everything
 // write_no_sync): cells are claimed with an atomic OR, entries popped with an atomic ADD, keep-alive is an atomic MIN and the
-// reposition vote is last-writer-wins.  The same atomics are used here; which thread wins is scheduling dependent, exactly as
-// on the reference's GPU.
+// reposition vote is last-writer-wins, so which thread wins is scheduling dependent.  Two schedules are built here:
+//  * the reference's atomics as they land (KJB_OPTION_ORDERED_CACHE_SCHEDULE = 0, the CPU emulator's default, where launches run in
+//    order; kjb_set_debug_serial runs them in launch order on the GPU too): the oracle's schedule, bit for bit;
+//  * ordered (the default on the GPU): the same decisions made independently of the order the threads run in, so that the
+//    same inputs give the same frames on every run.  A pass only reads the cache state it started with.  A claimed cell gets
+//    its entry at the start of the next cache chain, where the claims of all passes take the lowest free entries in cell
+//    order (k_ircache_det_*), and the winning vote of its claimers as its position at the chain's ageing; until then it
+//    reads as just allocated, which is what every lookup of it returned anyway.  The
+//    keep-alive of a lookup is applied there too.  Reposition votes keep the proposal whose hash is smallest (a 128-bit
+//    compare-and-swap), i.e. a uniform choice among the voters like the reference's reservoir vote, but one that does not
+//    depend on the order of the votes.  The precise lookups of the cache's own tracing passes read the per-entry reservoirs
+//    as they were when the pass started (`aux_prev`), not as the pass is rewriting them.
 #pragma once
+#include "kjb_context.h"
 #include "kjb_trace.cuh"
 
 namespace kjb {
@@ -37,10 +48,58 @@ KJB_DEV uint32_t atom_min(uint32_t* p, uint32_t v) { uint32_t c = *p; while (c >
 KJB_DEV uint32_t atom_max(uint32_t* p, uint32_t v) { uint32_t c = *p; while (c < v && !__atomic_compare_exchange_n(p, &c, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return c; }
 #endif
 
-// DEFINE_IRCACHE_BINDINGS (ircache/bindings.hlsl) + the aux buffer for IRCACHE_LOOKUP_PRECISE
+KJB_DEV uint32_t kjb_popc(uint32_t x) {
+#if defined(__CUDA_ARCH__)
+    return __popc(x);
+#else
+    return uint32_t(__builtin_popcount(x));
+#endif
+}
+// 128-bit compare-and-swap (sm_90); returns the value found
+KJB_DEV uint4 atom_cas128(float4* p, uint4 expected, uint4 desired) {
+#if defined(__CUDA_ARCH__)
+    unsigned long long lo, hi;
+    const unsigned long long elo = expected.x | (unsigned long long)expected.y << 32, ehi = expected.z | (unsigned long long)expected.w << 32;
+    const unsigned long long dlo = desired.x | (unsigned long long)desired.y << 32, dhi = desired.z | (unsigned long long)desired.w << 32;
+    asm volatile("{\n\t.reg .b128 e, d, r;\n\tmov.b128 e, {%2, %3};\n\tmov.b128 d, {%4, %5};\n\tatom.cas.b128 r, [%6], e, d;\n\tmov.b128 {%0, %1}, r;\n\t}"
+                 : "=l"(lo), "=l"(hi) : "l"(elo), "l"(ehi), "l"(dlo), "l"(dhi), "l"(p) : "memory");
+    return make_uint4(uint32_t(lo), uint32_t(lo >> 32), uint32_t(hi), uint32_t(hi >> 32));
+#else
+    unsigned __int128 e, d; memcpy(&e, &expected, 16); memcpy(&d, &desired, 16);
+    const unsigned __int128 r = __sync_val_compare_and_swap(reinterpret_cast<unsigned __int128*>(p), e, d);
+    uint4 out; memcpy(&out, &r, 16); return out;
+#endif
+}
+KJB_DEV bool u4_eq(uint4 a, uint4 b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
+KJB_DEV bool vertex_vote_beats(uint4 a, uint4 b) {   // an empty (all-zero) slot loses to any vote; else the smaller hash, then the smaller bits
+    if (b.x == 0u && b.y == 0u && b.z == 0u && b.w == 0u) return true;
+    const uint32_t ka = hash1(a.x ^ hash1(a.y ^ hash1(a.z ^ hash1(a.w)))), kb = hash1(b.x ^ hash1(b.y ^ hash1(b.z ^ hash1(b.w))));
+    if (ka != kb) return ka < kb;
+    if (a.x != b.x) return a.x < b.x;
+    if (a.y != b.y) return a.y < b.y;
+    if (a.z != b.z) return a.z < b.z;
+    return a.w < b.w;
+}
+// the slot ends up holding the winning vote of all the votes cast into it, whatever their order
+KJB_DEV void vertex_vote(float4* slot, float4 v) {
+    const uint4 nv = make_uint4(kjb_f2u(v.x), kjb_f2u(v.y), kjb_f2u(v.z), kjb_f2u(v.w));
+    uint4 cur = atom_cas128(slot, make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u));   // an atomic read
+    while (vertex_vote_beats(nv, cur)) {
+        const uint4 prev = atom_cas128(slot, cur, nv);
+        if (u4_eq(prev, cur)) return;
+        cur = prev;
+    }
+}
+
+// DEFINE_IRCACHE_BINDINGS (ircache/bindings.hlsl) + the aux buffer for IRCACHE_LOOKUP_PRECISE, + the scratch of the parallel schedule
 struct IrcacheBufs {
     uint32_t *meta, *pool, *reposition_count, *grid_meta, *entry_cell, *life;
     float4 *reposition_proposal, *spatial, *irradiance, *aux;
+    uint32_t* claim_rank = nullptr;      // per cell: RANK_COUNT - the lowest rank that claimed it since the last chain, 0 = unclaimed
+    float4* claim_vertex = nullptr;      // per cell: the winning reposition vote of its claimers
+    uint32_t* life_pending = nullptr;    // per entry: RECYCLE - the lowest life a lookup asked for, 0 = none
+    const float4* aux_prev = nullptr;    // per entry: its 32 reservoir + contribution texels as the pass found them
+    bool det = false;                    // the parallel schedule above
     KJB_DEV bool bound() const { return meta != nullptr; }
 };
 inline IrcacheBufs ircache_bufs(const kjb_ircache_bindings& b) {
@@ -125,11 +184,15 @@ KJB_DEV float eval_sh_geometrics(float4 sh, float3 normal) {   // lookup.hlsl:19
     return R0 * (a + (1.0f - a) * (p + 1.0f) * kjb_pow(q, p));
 }
 
+template <bool PRECISE>
+KJB_DEV float3 ircache_lookup_parallel(const Globals& g, const IrcacheBufs& b, float3 query_from_ws, float3 pt_ws, float3 normal_ws, uint32_t query_rank, uint32_t& rng, bool stochastic_interpolation);
+
 // IrcacheLookupParams::lookup (lookup.hlsl:76-311) with the maybe-allocating lookup it wraps (:19-74,:120-190).
 // PRECISE = IRCACHE_LOOKUP_PRECISE: sum the per-direction reservoirs instead of evaluating the SH (the cache's own tracing passes).
 template <bool PRECISE>
 KJB_DEV float3 ircache_lookup(const Globals& g, const IrcacheBufs& b, float3 query_from_ws, float3 pt_ws, float3 normal_ws, uint32_t query_rank, uint32_t& rng, bool stochastic_interpolation = false) {
     if (!b.bound()) return f3(0.0f);
+    if (b.det) return ircache_lookup_parallel<PRECISE>(g, b, query_from_ws, pt_ws, normal_ws, query_rank, rng, stochastic_interpolation);
     const kjb_frame_constants& fc = g.fc;
     bool allocated_by_us = false, just_allocated = false;
     // lookup.hlsl:80-86: the three rng draws sit in the arguments of select(), i.e. they happen whether or not interpolation is on
@@ -212,6 +275,96 @@ KJB_DEV float3 ircache_lookup(const Globals& g, const IrcacheBufs& b, float3 que
         }
     }
     return irradiance_sum;
+}
+
+// The same lookup on the parallel schedule (header comment): the same returned value and the same draws from `rng`; the cache
+// updates go where their order cannot matter.
+template <bool PRECISE>
+KJB_DEV float3 ircache_lookup_parallel(const Globals& g, const IrcacheBufs& b, float3 query_from_ws, float3 pt_ws, float3 normal_ws, uint32_t query_rank, uint32_t& rng, bool stochastic_interpolation) {
+    const kjb_frame_constants& fc = g.fc;
+    float3 jr; jr.x = rand01(rng); jr.y = rand01(rng); jr.z = rand01(rng);
+    const IrcacheCoord rc = ws_pos_to_ircache_coord(fc, pt_ws, normal_ws, stochastic_interpolation ? jr - 0.5f : f3(0.0f));
+    const uint32_t cell_idx = ircache_cell_idx(rc);
+    const float cell_diameter = ircache_grid_cell_diameter_in_cascade(rc.cascade);
+    float3 offset_towards_query = query_from_ws - pt_ws;
+    const float MAX_OFFSET = cell_diameter, MAX_OFFSET_AS_FRAC = 0.5f;
+    offset_towards_query = offset_towards_query * (MAX_OFFSET / kjb_max(MAX_OFFSET / MAX_OFFSET_AS_FRAC, length(offset_towards_query)));
+    IrcacheVertex new_entry; new_entry.position = pt_ws + offset_towards_query; new_entry.normal = normal_ws;
+
+    const uint32_t entry_flags = b.grid_meta[cell_idx * 2 + 1];
+    // no entry yet: unoccupied, or claimed (occupied + just allocated) and waiting for the next chain.  Every such lookup takes part in the
+    // claim, whether or not another one got there first: the claim's rank and position do not depend on who read the flags when.
+    if ((entry_flags & (IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED)) != IRCACHE_ENTRY_META_OCCUPIED) {
+        const int32_t* so = fc.ircache_cascades[rc.cascade].voxels_scrolled_this_frame;
+        const int c3[3] = {int(rc.cx), int(rc.cy), int(rc.cz)};
+        bool was_just_scrolled_in = false;
+        for (int k = 0; k < 3; ++k) was_just_scrolled_in = was_just_scrolled_in || (so[k] > 0 ? (c3[k] + so[k] >= int(IRCACHE_CASCADE_SIZE)) : (c3[k] < -so[k]));
+        if (!(query_rank >= IRCACHE_ENTRY_RANK_COUNT || (was_just_scrolled_in && query_rank > 0))) {   // claim: the entry comes with the next chain
+            atom_or(&b.grid_meta[cell_idx * 2 + 1], IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED);
+            atom_max(&b.claim_rank[cell_idx], IRCACHE_ENTRY_RANK_COUNT - query_rank);
+            vertex_vote(&b.claim_vertex[cell_idx], pack_vertex(new_entry));
+        }
+        return f3(0.0f);
+    }
+
+    const uint32_t entry_idx = b.grid_meta[cell_idx * 2 + 0];
+    float3 irradiance = f3(0.0f);
+    if (PRECISE) {
+        float weight_sum = 0;
+        for (uint32_t octa_idx = 0; octa_idx < IRCACHE_OCTA_DIMS2; ++octa_idx) {
+            const float4 ra = b.aux_prev[entry_idx * 32u + octa_idx];
+            const Reservoir r = Reservoir::from_raw(u2(kjb_f2u(ra.x), kjb_f2u(ra.y)));
+            const float3 dir = SampleParams::from_raw(r.payload).direction();
+            const float wt = dot(dir, normal_ws);
+            if (wt > 0.0f) {
+                const float4 contrib = b.aux_prev[entry_idx * 32u + IRCACHE_OCTA_DIMS2 + octa_idx];
+                irradiance += xyz(contrib) * wt * contrib.w;
+                weight_sum += wt;
+            }
+        }
+        irradiance = irradiance / kjb_max(1.0f, weight_sum);
+    } else {
+        irradiance.x += eval_sh_geometrics(b.irradiance[entry_idx * 3 + 0], normal_ws);
+        irradiance.y += eval_sh_geometrics(b.irradiance[entry_idx * 3 + 1], normal_ws);
+        irradiance.z += eval_sh_geometrics(b.irradiance[entry_idx * 3 + 2], normal_ws);
+    }
+    irradiance = vmax(f3(0.0f), irradiance);
+    const uint32_t prev_life = b.life[entry_idx];   // not written while a pass runs: the keep-alive waits in life_pending
+    if (prev_life < IRCACHE_ENTRY_LIFE_RECYCLE) {
+        const uint32_t new_life = ircache_entry_life_for_rank(query_rank);
+        if (new_life < prev_life) atom_max(&b.life_pending[entry_idx], IRCACHE_ENTRY_LIFE_RECYCLE - new_life);
+        if (query_rank <= ircache_entry_life_to_rank(prev_life)) {
+            atom_add(&b.reposition_count[entry_idx], 1u);
+            (void)rand01(rng);   // the serial schedule's dart: drawn all the same, so that the caller's stream does not depend on the schedule
+            vertex_vote(&b.reposition_proposal[entry_idx], pack_vertex(new_entry));
+        }
+    }
+    return irradiance;
+}
+
+// the ordered schedule's scratch of the cache whose life buffer is `life` (allocated zeroed on first use); false = the reference's atomics
+inline bool ircache_parallel_scratch(kjb_context* c, const void* life, kjb_context::IrcacheScratch& out) {
+    if (c->debug_serial || !c->ordered_cache || !life) return false;
+    auto it = c->ircache_scratch.find(life);
+    if (it == c->ircache_scratch.end()) {
+        kjb_context::IrcacheScratch s;
+        s.claim_rank = dev_alloc(4ull * KJB_IRCACHE_GRID_CELLS); s.claim_vertex = dev_alloc(16ull * KJB_IRCACHE_GRID_CELLS);
+        s.life_pending = dev_alloc(4ull * KJB_IRCACHE_MAX_ENTRIES); s.scan = dev_alloc(4ull * (KJB_IRCACHE_MAX_ENTRIES + KJB_IRCACHE_GRID_CELLS / 32));
+        s.claim_bits = dev_alloc(4ull * KJB_IRCACHE_GRID_CELLS / 32); s.aux_prev = dev_alloc(16ull * 32 * KJB_IRCACHE_MAX_ENTRIES); s.entry_vertex = dev_alloc(16ull * KJB_IRCACHE_MAX_ENTRIES);
+        if (!s.claim_rank || !s.claim_vertex || !s.life_pending || !s.scan || !s.claim_bits || !s.aux_prev || !s.entry_vertex) {
+            dev_free(s.claim_rank); dev_free(s.claim_vertex); dev_free(s.life_pending); dev_free(s.scan); dev_free(s.claim_bits); dev_free(s.aux_prev); dev_free(s.entry_vertex);
+            return false;
+        }
+        it = c->ircache_scratch.emplace(life, s).first;
+    }
+    out = it->second;
+    return true;
+}
+inline void ircache_attach_parallel(kjb_context* c, IrcacheBufs& b) {
+    kjb_context::IrcacheScratch s;
+    if (!b.bound() || !ircache_parallel_scratch(c, b.life, s)) return;
+    b.claim_rank = (uint32_t*)s.claim_rank; b.claim_vertex = (float4*)s.claim_vertex; b.life_pending = (uint32_t*)s.life_pending; b.aux_prev = (const float4*)s.aux_prev;
+    b.det = true;
 }
 
 }  // namespace kjb

@@ -1,4 +1,4 @@
-// Irradiance cache (ircache) as sm_100a kernels — one kernel per render-graph pass of
+// Irradiance cache (ircache) as sm_90a kernels — one kernel per render-graph pass of
 // crates/lib/kajiya/src/renderers/ircache.rs, shader sources under /root/reference/assets/shaders/ircache/.
 // All passes are 1-D over cache entries / grid cells.  The reference's indirect dispatches become fixed-size launches that
 // early-out on the counters in `meta_buf` (like the reference's own fixed-size validate/trace dispatches, ircache.rs:438-476),
@@ -27,7 +27,8 @@ KJB_KERNEL(256) k_ircache_clear_pool(uint32_t* pool, uint32_t* life, Rows kjb_ro
 }
 
 // ------------------------------------------------------------------ I2 scroll_cascades.hlsl:36-69
-KJB_DEV void ircache_scroll_cell(const Globals& g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta, uint32_t dst_cell_idx) {
+KJB_DEV void ircache_scroll_cell(const Globals& g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta, uint32_t dst_cell_idx,
+                                 bool parallel = false) {
     const uint32_t x = dst_cell_idx & 31u, y = (dst_cell_idx >> 5) & 31u, z = (dst_cell_idx >> 10) & 31u, cascade = dst_cell_idx >> 15;
     const int32_t* sb = g.fc.ircache_cascades[cascade].voxels_scrolled_this_frame;
     const uint32_t ox = x - uint32_t(sb[0]), oy = y - uint32_t(sb[1]), oz = z - uint32_t(sb[2]);
@@ -38,7 +39,7 @@ KJB_DEV void ircache_scroll_cell(const Globals& g, const uint32_t* gm, uint32_t*
             life[entry_idx] = IRCACHE_ENTRY_LIFE_RECYCLED;
             for (uint32_t i = 0; i < IRCACHE_IRRADIANCE_STRIDE; ++i) irradiance[entry_idx * IRCACHE_IRRADIANCE_STRIDE + i] = f4(0.0f);
             const uint32_t entry_alloc_count = atom_add(&meta[IRCACHE_META_ALLOC_COUNT], uint32_t(-1));
-            pool[entry_alloc_count - 1] = entry_idx;
+            if (!parallel) pool[entry_alloc_count - 1] = entry_idx;   // the parallel schedule rebuilds the pool in entry order instead
         }
     }
     const uint32_t sx = x + uint32_t(sb[0]), sy = y + uint32_t(sb[1]), sz = z + uint32_t(sb[2]);
@@ -49,8 +50,9 @@ KJB_DEV void ircache_scroll_cell(const Globals& g, const uint32_t* gm, uint32_t*
         if (m1 & IRCACHE_ENTRY_META_OCCUPIED) entry_cell[m0] = dst_cell_idx;
     } else { gm2[dst_cell_idx * 2] = 0; gm2[dst_cell_idx * 2 + 1] = 0; }
 }
-KJB_KERNEL(256) k_ircache_scroll_cascades(const __grid_constant__ Globals g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta, Rows kjb_rows) {
-    const uint32_t i = tid1d(); if (i < KJB_IRCACHE_GRID_CELLS) ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i);
+KJB_KERNEL(256) k_ircache_scroll_cascades(const __grid_constant__ Globals g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta,
+                                          uint32_t parallel, Rows kjb_rows) {
+    const uint32_t i = tid1d(); if (i < KJB_IRCACHE_GRID_CELLS) ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i, parallel != 0);
 }
 // `_serial` twins (kjb_set_debug_serial): ONE thread walks the logical threads in launch order — the deterministic schedule the
 // CPU oracle uses, so the racy cache passes can be compared bit for bit on the real GPU (slow; test / repro aid only)
@@ -76,7 +78,7 @@ KJB_KERNEL(32) k_ircache_prepare_trace_args(uint32_t* meta, uint32_t* args, Rows
 
 // ------------------------------------------------------------------ I4 age_ircache_entries.hlsl:55-94
 KJB_DEV void ircache_age_entry(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, uint32_t* pool, float4* spatial, float4* proposal, uint32_t* proposal_count,
-                               float4* irradiance, uint32_t* occupancy, uint32_t entry_idx) {
+                               float4* irradiance, uint32_t* occupancy, uint32_t entry_idx, float4* entry_vertex = nullptr) {
     const uint32_t total_entry_count = meta[IRCACHE_META_ENTRY_COUNT];
     if (entry_idx >= (total_entry_count + 63u) / 64u * 64u) return;   // the reference dispatches ceil(entry_count / 64) groups
     if (entry_idx < total_entry_count) {
@@ -90,11 +92,18 @@ KJB_DEV void ircache_age_entry(uint32_t* meta, uint32_t* gm, uint32_t* entry_cel
                 life[entry_idx] = IRCACHE_ENTRY_LIFE_RECYCLED;
                 for (uint32_t i = 0; i < IRCACHE_IRRADIANCE_STRIDE; ++i) irradiance[entry_idx * IRCACHE_IRRADIANCE_STRIDE + i] = f4(0.0f);
                 const uint32_t entry_alloc_count = atom_add(&meta[IRCACHE_META_ALLOC_COUNT], uint32_t(-1));
-                pool[entry_alloc_count - 1] = entry_idx;
+                if (!entry_vertex) pool[entry_alloc_count - 1] = entry_idx;
                 atom_and(&gm[entry_cell[entry_idx] * 2 + 1], ~(IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED));
             }
         }
-        spatial[entry_idx] = proposal[entry_idx];   // flush the reposition proposal (IRCACHE_USE_POSITION_VOTING)
+        if (!entry_vertex) {
+            spatial[entry_idx] = proposal[entry_idx];   // flush the reposition proposal (IRCACHE_USE_POSITION_VOTING)
+        } else {                                        // parallel schedule: votes compete for an emptied slot, no vote = no move; a new entry starts at its claimers' vote
+            float4 v = proposal[entry_idx];
+            if (!(kjb_f2u(v.x) | kjb_f2u(v.y) | kjb_f2u(v.z) | kjb_f2u(v.w))) v = entry_vertex[entry_idx];
+            if (kjb_f2u(v.x) | kjb_f2u(v.y) | kjb_f2u(v.z) | kjb_f2u(v.w)) spatial[entry_idx] = v;
+            proposal[entry_idx] = f4(0.0f); entry_vertex[entry_idx] = f4(0.0f);
+        }
         proposal_count[entry_idx] = 0;
     } else {
         spatial[entry_idx] = f4(0.0f);
@@ -103,13 +112,66 @@ KJB_DEV void ircache_age_entry(uint32_t* meta, uint32_t* gm, uint32_t* entry_cel
     occupancy[entry_idx] = (entry_idx < total_entry_count && is_ircache_entry_life_valid(l2)) ? 1u : 0u;
 }
 KJB_KERNEL(256) k_ircache_age(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, uint32_t* pool, float4* spatial, float4* proposal, uint32_t* proposal_count,
-                              float4* irradiance, uint32_t* occupancy, Rows kjb_rows) {
-    const uint32_t i = tid1d(); if (i < MAX_ENTRIES) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i);
+                              float4* irradiance, uint32_t* occupancy, float4* entry_vertex, Rows kjb_rows) {
+    const uint32_t i = tid1d(); if (i < MAX_ENTRIES) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i, entry_vertex);
 }
 KJB_KERNEL(32) k_ircache_age_serial(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, uint32_t* pool, float4* spatial, float4* proposal, uint32_t* proposal_count,
                                     float4* irradiance, uint32_t* occupancy, Rows kjb_rows) {
     if (tid1d() != 0) return;
     for (uint32_t i = 0; i < MAX_ENTRIES; ++i) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i);
+}
+
+// ------------------------------------------------------------------ the parallel schedule's entry assignment (kjb_ircache.cuh), at the start of a chain
+// per entry: apply the keep-alive the lookups asked for, mark the free entries (life RECYCLED, the ones the pool holds)
+KJB_KERNEL(256) k_ircache_det_free(uint32_t* life, uint32_t* life_pending, uint32_t* free_scan, Rows kjb_rows) {
+    const uint32_t e = tid1d(); if (e >= MAX_ENTRIES) return;
+    uint32_t l = life[e];
+    const uint32_t p = life_pending[e];
+    if (p) {
+        const uint32_t nl = IRCACHE_ENTRY_LIFE_RECYCLE - p;
+        if (l < IRCACHE_ENTRY_LIFE_RECYCLE && nl < l) life[e] = l = nl;
+        life_pending[e] = 0;
+    }
+    free_scan[e] = l == IRCACHE_ENTRY_LIFE_RECYCLED ? 1u : 0u;
+}
+// per entry (after the scan): the free entries in ascending order fill the pool above the allocated count, where the pops take them from
+KJB_KERNEL(256) k_ircache_det_pool(const uint32_t* free_scan, uint32_t* pool, uint32_t* meta, Rows kjb_rows) {
+    const uint32_t e = tid1d(); if (e >= MAX_ENTRIES) return;
+    const uint32_t base = MAX_ENTRIES - free_scan[MAX_ENTRIES - 1];
+    if (e == 0) meta[IRCACHE_META_ALLOC_COUNT] = base;
+    if (free_scan[e] != (e ? free_scan[e - 1] : 0u)) pool[base + free_scan[e] - 1] = e;
+}
+// per 32 cells: which were claimed, and how many
+KJB_KERNEL(256) k_ircache_det_claims(const uint32_t* claim_rank, uint32_t* claim_bits, uint32_t* claim_scan, Rows kjb_rows) {
+    const uint32_t w = tid1d(); if (w >= KJB_IRCACHE_GRID_CELLS / 32) return;
+    uint32_t m = 0;
+    for (uint32_t k = 0; k < 32; ++k) m |= (claim_rank[w * 32 + k] ? 1u : 0u) << k;
+    claim_bits[w] = m; claim_scan[w] = kjb_popc(m);
+}
+// per cell (after the scan of the claim counts): the n-th claimed cell in cell order takes the n-th free entry; beyond the pool the claim is dropped
+KJB_KERNEL(256) k_ircache_det_assign(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, const uint32_t* pool, float4* entry_vertex, uint32_t* claim_rank, float4* claim_vertex,
+                                     const uint32_t* free_scan, const uint32_t* claim_bits, const uint32_t* claim_scan, Rows kjb_rows) {
+    const uint32_t cell = tid1d(); if (cell >= KJB_IRCACHE_GRID_CELLS) return;
+    const uint32_t w = cell >> 5, k = cell & 31u, m = claim_bits[w];
+    if (!((m >> k) & 1u)) return;
+    const uint32_t n = (w ? claim_scan[w - 1] : 0u) + kjb_popc(m & ((1u << k) - 1u));
+    const uint32_t free_count = free_scan[MAX_ENTRIES - 1];
+    const uint32_t rank = IRCACHE_ENTRY_RANK_COUNT - claim_rank[cell];
+    const float4 v = claim_vertex[cell];
+    claim_rank[cell] = 0; claim_vertex[cell] = f4(0.0f);
+    if (n >= free_count) { atom_and(&gm[cell * 2 + 1], ~(IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED)); return; }
+    const uint32_t entry_idx = pool[MAX_ENTRIES - free_count + n];
+    atom_max(&meta[IRCACHE_META_ENTRY_COUNT], entry_idx + 1);
+    atom_add(&meta[IRCACHE_META_ALLOC_COUNT], 1u);
+    life[entry_idx] = ircache_entry_life_for_rank(rank);
+    entry_cell[entry_idx] = cell;
+    gm[cell * 2 + 0] = entry_idx;
+    entry_vertex[entry_idx] = v;
+}
+// per entry: its reservoirs and contributions as the coming pass finds them, for the precise lookups of that pass
+KJB_KERNEL(256) k_ircache_det_snapshot_aux(const uint32_t* meta, const float4* aux, float4* aux_prev, Rows kjb_rows) {
+    const uint32_t i = tid1d(), e = i / 32u; if (e >= MAX_ENTRIES || e >= meta[IRCACHE_META_ENTRY_COUNT]) return;
+    aux_prev[i] = aux[e * IRCACHE_AUX_STRIDE + i % 32u];
 }
 
 // ------------------------------------------------------------------ I5 prefix_scan/*.hlsl: inclusive scan of <= 64 Ki u32 in one CTA
@@ -400,7 +462,8 @@ KJB_KERNEL(256) k_ircache_export_requests(IrcacheBufs b, uint32_t* block, uint32
     const uint32_t slot = atom_add(&block[0], 1u);            // the header may end up above max_records: readers clamp
     if (slot >= max_records) return;
     uint32_t* rec = block + 4 + slot * 8u;
-    const float4 v = b.reposition_proposal[e];
+    float4 v = b.reposition_proposal[e];
+    if (!(kjb_f2u(v.x) | kjb_f2u(v.y) | kjb_f2u(v.z) | kjb_f2u(v.w))) v = b.spatial[e];   // no vote yet (parallel schedule): where the entry is
     rec[0] = b.entry_cell[e]; rec[1] = life; rec[2] = b.reposition_count[e]; rec[3] = 0u;
     rec[4] = kjb_f2u(v.x); rec[5] = kjb_f2u(v.y); rec[6] = kjb_f2u(v.z); rec[7] = kjb_f2u(v.w);
 }
@@ -413,6 +476,13 @@ KJB_KERNEL(256) k_ircache_merge_requests(IrcacheBufs b, const uint32_t* block, u
     const uint32_t cell_idx = rec[0], life_r = rec[1], count_r = rec[2];
     if (cell_idx >= KJB_IRCACHE_GRID_CELLS || !is_ircache_entry_life_valid(life_r)) return;
     const float4 vote = f4(kjb_u2f(rec[4]), kjb_u2f(rec[5]), kjb_u2f(rec[6]), kjb_u2f(rec[7]));
+    if (b.det && (b.grid_meta[cell_idx * 2 + 1] & (IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED)) != IRCACHE_ENTRY_META_OCCUPIED) {
+        // parallel schedule: a cell without an entry yet is claimed like a lookup claims it, and gets its entry with the coming chain
+        atom_or(&b.grid_meta[cell_idx * 2 + 1], IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED);
+        atom_max(&b.claim_rank[cell_idx], IRCACHE_ENTRY_RANK_COUNT - ircache_entry_life_to_rank(life_r));
+        vertex_vote(&b.claim_vertex[cell_idx], vote);
+        return;
+    }
     bool fresh = false;
     if ((b.grid_meta[cell_idx * 2 + 1] & IRCACHE_ENTRY_META_OCCUPIED) == 0) {      // no local ray asked for this cell: allocate it as the lookup would (lookup.hlsl:19-74)
         const uint32_t prev = atom_or(&b.grid_meta[cell_idx * 2 + 1], IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED);
@@ -455,6 +525,10 @@ int kjb_pass_ircache_clear_pool(kjb_context* c, const kjb_ircache_clear_pool_arg
     const char* P = "clear ircache pool"; BUF(a->pool_buf, uint32_t, MAX_ENTRIES, "pool_buf"); BUF(a->life_buf, uint32_t, MAX_ENTRIES, "life_buf");
     NO_SCISSOR;
     KJB_LAUNCH(c, k_ircache_clear_pool, DIMS1D(MAX_ENTRIES, 256), U32P(a->pool_buf), U32P(a->life_buf));
+    kjb_context::IrcacheScratch s;   // an emptied cache has no pending claims or keep-alives
+    if (ircache_parallel_scratch(c, a->life_buf.data, s) && (dev_memset(c, s.claim_rank, 0, 4ull * KJB_IRCACHE_GRID_CELLS) || dev_memset(c, s.claim_vertex, 0, 16ull * KJB_IRCACHE_GRID_CELLS)
+                                                               || dev_memset(c, s.life_pending, 0, 4ull * MAX_ENTRIES) || dev_memset(c, s.entry_vertex, 0, 16ull * MAX_ENTRIES)))
+        return c->fail(std::string(P) + ": memset failed");
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_ircache_scroll_cascades(kjb_context* c, const kjb_ircache_scroll_cascades_args* a) {
@@ -463,10 +537,21 @@ int kjb_pass_ircache_scroll_cascades(kjb_context* c, const kjb_ircache_scroll_ca
     BUF(a->entry_cell_buf, uint32_t, MAX_ENTRIES, "entry_cell_buf"); BUF(a->irradiance_buf, float4, 3 * MAX_ENTRIES, "irradiance_buf"); BUF(a->life_buf, uint32_t, MAX_ENTRIES, "life_buf");
     BUF(a->pool_buf, uint32_t, MAX_ENTRIES, "pool_buf"); BUF(a->meta_buf, uint32_t, 8, "meta_buf");
     NO_SCISSOR;
+    kjb_context::IrcacheScratch s;
+    if (ircache_parallel_scratch(c, a->life_buf.data, s)) {   // the claims of the last frame's passes take their entries (kjb_ircache.cuh)
+        uint32_t* free_scan = (uint32_t*)s.scan; uint32_t* claim_scan = free_scan + MAX_ENTRIES;
+        KJB_LAUNCH(c, k_ircache_det_free, DIMS1D(MAX_ENTRIES, 256), U32P(a->life_buf), (uint32_t*)s.life_pending, free_scan);
+        KJB_LAUNCH_SYNC(c, k_inclusive_prefix_scan, KJB_DIMS(dim3(1), dim3(1024)), free_scan, MAX_ENTRIES);
+        KJB_LAUNCH(c, k_ircache_det_pool, DIMS1D(MAX_ENTRIES, 256), (const uint32_t*)free_scan, U32P(a->pool_buf), U32P(a->meta_buf));
+        KJB_LAUNCH(c, k_ircache_det_claims, DIMS1D(KJB_IRCACHE_GRID_CELLS / 32, 256), (const uint32_t*)s.claim_rank, (uint32_t*)s.claim_bits, claim_scan);
+        KJB_LAUNCH_SYNC(c, k_inclusive_prefix_scan, KJB_DIMS(dim3(1), dim3(1024)), claim_scan, KJB_IRCACHE_GRID_CELLS / 32);
+        KJB_LAUNCH(c, k_ircache_det_assign, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), (const uint32_t*)U32P(a->pool_buf),
+                   (float4*)s.entry_vertex, (uint32_t*)s.claim_rank, (float4*)s.claim_vertex, (const uint32_t*)free_scan, (const uint32_t*)s.claim_bits, (const uint32_t*)claim_scan);
+    }
     if (c->debug_serial) KJB_LAUNCH(c, k_ircache_scroll_cascades_serial, DIMS1D(1, 32), c->g, U32P(a->grid_meta_buf), U32P(a->grid_meta_buf2), U32P(a->entry_cell_buf), F4P(a->irradiance_buf),
                        U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf));
     else KJB_LAUNCH_ORDERED(c, k_ircache_scroll_cascades, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), c->g, U32P(a->grid_meta_buf), U32P(a->grid_meta_buf2), U32P(a->entry_cell_buf), F4P(a->irradiance_buf),
-                       U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf));
+                       U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf), ircache_parallel_scratch(c, a->life_buf.data, s) ? 1u : 0u);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_ircache_prepare_age_dispatch_args(kjb_context* c, const kjb_ircache_dispatch_args_args* a) {
@@ -490,8 +575,12 @@ int kjb_pass_ircache_age_entries(kjb_context* c, const kjb_ircache_age_args* a) 
     NO_SCISSOR;
     if (c->debug_serial) KJB_LAUNCH(c, k_ircache_age_serial, DIMS1D(1, 32), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
                        F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf));
-    else KJB_LAUNCH_ORDERED(c, k_ircache_age, DIMS1D(MAX_ENTRIES, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
-                       F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf));
+    else {
+        kjb_context::IrcacheScratch s;
+        float4* entry_vertex = ircache_parallel_scratch(c, a->life_buf.data, s) ? (float4*)s.entry_vertex : nullptr;
+        KJB_LAUNCH_ORDERED(c, k_ircache_age, DIMS1D(MAX_ENTRIES, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
+                           F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf), entry_vertex);
+    }
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_inclusive_prefix_scan_u32(kjb_context* c, const kjb_prefix_scan_args* a) {
@@ -535,10 +624,16 @@ static int check_trace_args(kjb_context* c, const char* P, const kjb_ircache_tra
     if (!c->tlas_valid) return c->fail(std::string(P) + ": no acceleration structure (call kjb_rebuild_tlas)");
     b.meta = U32P(a->meta_buf); b.pool = U32P(a->pool_buf); b.reposition_count = U32P(a->reposition_proposal_count_buf); b.grid_meta = U32P(a->grid_meta_buf); b.entry_cell = U32P(a->entry_cell_buf);
     b.life = U32P(a->life_buf); b.reposition_proposal = F4P(a->reposition_proposal_buf); b.spatial = F4P(a->spatial_buf); b.irradiance = nullptr; b.aux = F4P(a->aux_buf);   // precise lookups read the per-entry reservoirs, not the SH
+    ircache_attach_parallel(c, b);
     return 0;
+}
+static void snapshot_aux(kjb_context* c, const IrcacheBufs& b) {   // parallel schedule: what the pass's precise lookups read
+    NO_SCISSOR;
+    if (b.det) KJB_LAUNCH(c, k_ircache_det_snapshot_aux, DIMS1D(MAX_ENTRIES * 32u, 256), (const uint32_t*)b.meta, (const float4*)b.aux, (float4*)b.aux_prev);
 }
 int kjb_pass_ircache_validate(kjb_context* c, const kjb_ircache_trace_args* a) {
     const char* P = "ircache validate"; IrcacheBufs b; if (check_trace_args(c, P, a, b)) return 1;
+    snapshot_aux(c, b);
     NO_SCISSOR;
     if (c->debug_serial) KJB_LAUNCH(c, k_ircache_validate_serial, DIMS1D(1, 32), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
     else KJB_LAUNCH_ORDERED(c, k_ircache_validate, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
@@ -546,6 +641,7 @@ int kjb_pass_ircache_validate(kjb_context* c, const kjb_ircache_trace_args* a) {
 }
 int kjb_pass_ircache_trace(kjb_context* c, const kjb_ircache_trace_args* a) {
     const char* P = "ircache trace"; IrcacheBufs b; if (check_trace_args(c, P, a, b)) return 1;
+    snapshot_aux(c, b);
     NO_SCISSOR;
     if (c->debug_serial) KJB_LAUNCH(c, k_ircache_trace_serial, DIMS1D(1, 32), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
     else KJB_LAUNCH_ORDERED(c, k_ircache_trace, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
@@ -578,7 +674,8 @@ int kjb_pass_ircache_merge_requests(kjb_context* c, const kjb_ircache_share_args
     BUF(a->block, uint8_t, KJB_IRCACHE_SHARE_BLOCK_BYTES(uint64_t(a->max_records)), "block");
     if (a->max_records == 0) return 0;
     NO_SCISSOR;
-    KJB_LAUNCH_ORDERED(c, k_ircache_merge_requests, DIMS1D(a->max_records, 256), ircache_bufs(a->ircache), (const uint32_t*)a->block.data, a->max_records, a->seed);
+    IrcacheBufs b = ircache_bufs(a->ircache); ircache_attach_parallel(c, b);
+    KJB_LAUNCH_ORDERED(c, k_ircache_merge_requests, DIMS1D(a->max_records, 256), b, (const uint32_t*)a->block.data, a->max_records, a->seed);
     KJB_PASS_EPILOGUE(c, P);
 }
 

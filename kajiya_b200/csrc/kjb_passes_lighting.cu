@@ -1,4 +1,4 @@
-// Lighting composite (SURVEY §8f N4) as sm_100a kernels: "trace shadow mask" (renderers/shadows.rs:10-35,
+// Lighting composite (SURVEY §8f N4) as sm_90a kernels: "trace shadow mask" (renderers/shadows.rs:10-35,
 // rt/trace_sun_shadow_mask.rgen.hlsl) and "light gbuffer" (renderers/deferred.rs:8-43, light_gbuffer.hlsl).
 #include "kjb_context.h"
 

@@ -1,4 +1,4 @@
-// Input producers and utility passes as sm_100a kernels (one thread per texel, 32x8 blocks => each warp touches one
+// Input producers and utility passes as sm_90a kernels (one thread per texel, 32x8 blocks => each warp touches one
 // contiguous row segment: 128..512 B per request depending on the texel size).
 #include "kjb_context.h"
 

@@ -1,9 +1,9 @@
-// Ray-traced diffuse GI (rtdgi) as sm_100a kernels — one kernel per render-graph pass of
+// Ray-traced diffuse GI (rtdgi) as sm_90a kernels — one kernel per render-graph pass of
 // crates/lib/kajiya/src/renderers/rtdgi.rs, shader sources under /root/reference/assets/shaders/rtdgi/.
 // Thread mapping: 32x8 blocks on the pass's pixel grid (a warp = 32 consecutive pixels of one row, so the 4/8/16-byte
 // texels of every bound image are fetched as 128/256/512-byte contiguous requests); the two ray-tracing passes use
 // 16x8 blocks (register pressure of the traversal stack + BRDF state).  Neighbourhood taps go through L1/L2: the
-// half-res working set at 1080p (~40 MB for all ReSTIR state) is L2-resident on B200 (126 MB).
+// half-res working set at 1080p (~40 MB for all ReSTIR state) is largely L2-resident on H100 (50 MB).
 #include "kjb_context.h"
 #include "kjb_ircache.cuh"
 
@@ -181,7 +181,7 @@ KJB_DEV void rtdgi_validate_px(const Globals& g, const Img& half_view_normal_tex
     st_r8u(out_tex, x, y, invalidity);
 }
 #ifndef KJB_OCC_VALIDATE
-#define KJB_OCC_VALIDATE 8   /* 72 -> 64 registers: 147 -> 137 us at 1080p (profiles/r02n_variants.txt) */
+#define KJB_OCC_VALIDATE 8   /* 64 registers */
 #endif
 KJB_KERNEL_OCC(128, KJB_OCC_VALIDATE) k_rtdgi_validate(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, ImgW reservoir_tex, Img reservoir_ray_history_tex,
                                  Img sky_cube_tex, ImgW irradiance_history_tex, Img ray_orig_history_tex, ImgW out_tex, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
@@ -235,7 +235,7 @@ KJB_DEV void rtdgi_trace_px(const Globals& g, const Img& half_view_normal_tex, c
     st_r8u(inv_out, x, y, ld_r8u(inv_in, rx, ry));
 }
 #ifndef KJB_OCC_TRACE
-#define KJB_OCC_TRACE 8   /* 64 registers: 377 (4 blocks) / 356 (6) / 331 us (8) at 1080p atrium (profiles/r02j_variants.txt) */
+#define KJB_OCC_TRACE 8   /* 64 registers */
 #endif
 KJB_KERNEL_OCC(128, KJB_OCC_TRACE) k_rtdgi_trace(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, Img reprojection_tex, Img sky_cube_tex,
                               ImgW cand_irr, ImgW cand_normal, ImgW cand_hit, Img inv_in, ImgW inv_out, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
@@ -315,7 +315,7 @@ struct RestirTemporalImgs {
     ImgW radiance_out_tex, ray_orig_output_tex, ray_output_tex, hit_normal_output_tex, reservoir_out_tex, candidate_out_tex, temporal_reservoir_packed_tex;
 };
 #ifndef KJB_OCC_RESTIR_TEMPORAL
-#define KJB_OCC_RESTIR_TEMPORAL 4   /* 64 registers: 45 -> 36 us */
+#define KJB_OCC_RESTIR_TEMPORAL 4   /* 64 registers */
 #endif
 KJB_KERNEL_OCC(256, KJB_OCC_RESTIR_TEMPORAL) k_rtdgi_restir_temporal(const __grid_constant__ Globals g, RestirTemporalImgs t, float4 gts, float4* positions, Rows kjb_rows) {
     KJB_PX; if (x >= t.radiance_out_tex.w || y >= t.radiance_out_tex.h) return;
@@ -469,7 +469,7 @@ static PosView ensure_positions(kjb_context* c, kjb_context::PosCache& pc, uint6
 // ------------------------------------------------------------------ D7 restir_spatial.hlsl:48-372 + occlusion_raymarch.hlsl:69-146
 KJB_DEV float normal_influence_nonlinearity(float x, float b) { return x < -b ? 0.0f : (x + b) * (x + b) / (4 * b); }
 #ifndef KJB_OCC_RESTIR_SPATIAL
-#define KJB_OCC_RESTIR_SPATIAL 1   /* 74 registers; capping at 64 / 48 costs 5 % / 13 % */
+#define KJB_OCC_RESTIR_SPATIAL 1   /* 77 registers, uncapped */
 #endif
 KJB_KERNEL_OCC(256, KJB_OCC_RESTIR_SPATIAL) k_rtdgi_restir_spatial(const __grid_constant__ Globals g, Img reservoir_input_tex, Img half_view_normal_tex, Img half_depth_tex, Img half_ssao_tex, Img temporal_reservoir_packed_tex,
                                        ImgW reservoir_output_tex, float4 gts, float4 ots, uint32_t pass_idx, uint32_t perform_occlusion_raymarch, uint32_t importance_only, PosView pos_a, PosView pos_b, Rows kjb_rows) {
@@ -631,7 +631,7 @@ KJB_DEV float ggx_ndf_unnorm(float a2, float cos_theta) { const float ds = cos_t
 struct ResolveImgs { Img radiance_tex, reservoir_input_tex, gbuffer_tex, depth_tex, half_view_normal_tex, half_depth_tex, ssao_tex, candidate_radiance_tex, candidate_hit_tex, temporal_reservoir_packed_tex; };
 struct PowTable4 { float v[4]; };   // v[i] = pow(float(i), 0.666), host-evaluated
 #ifndef KJB_OCC_RESTIR_RESOLVE
-#define KJB_OCC_RESTIR_RESOLVE 5   /* 48 registers, 5 blocks/SM: 117 -> 112 us at 1080p (profiles/r01r_variants.txt) */
+#define KJB_OCC_RESTIR_RESOLVE 5   /* 48 registers, 5 blocks/SM */
 #endif
 KJB_KERNEL_OCC(256, KJB_OCC_RESTIR_RESOLVE) k_rtdgi_restir_resolve(const __grid_constant__ Globals g, ResolveImgs t, ImgW irradiance_output_tex, float4 gts, float4 ots, PowTable4 pw, PosView pos_a, PosView pos_b, Rows kjb_rows) {
     KJB_PX; if (x >= irradiance_output_tex.w || y >= irradiance_output_tex.h) return;
@@ -860,6 +860,7 @@ static int check_ircache_bindings(kjb_context* c, const char* P, const kjb_ircac
         && b.reposition_proposal_count_buf.data && b.reposition_proposal_count_buf.size_bytes >= 4 * E;
     if (!ok) return c->fail(std::string(P) + ": irradiance cache bindings are incomplete or too small");
     out = ircache_bufs(b);
+    ircache_attach_parallel(c, out);
     return 0;
 }
 

@@ -1,4 +1,4 @@
-// Ray-traced specular reflections (rtr) as sm_100a kernels — one kernel per render-graph pass of
+// Ray-traced specular reflections (rtr) as sm_90a kernels — one kernel per render-graph pass of
 // crates/lib/kajiya/src/renderers/rtr.rs, shader sources under /root/reference/assets/shaders/rtr/ (settings frozen to rtr_settings.hlsl).
 // Thread mapping as in kjb_passes_rtdgi.cu: 32x8 blocks on the pass's pixel grid, 8x16 for the two ray-tracing passes (a warp = an 8x4 pixel patch).
 #include "kjb_context.h"
@@ -167,7 +167,7 @@ KJB_DEV void rtr_trace_px(const Globals& g, const RtrTraceImgs& t, const BlueNoi
     }
 }
 #ifndef KJB_OCC_RTR_TRACE
-#define KJB_OCC_RTR_TRACE 8   /* 80 -> 64 registers: 296 -> 276 us at 1080p (profiles/r02n_variants.txt) */
+#define KJB_OCC_RTR_TRACE 8   /* 80 -> 64 registers */
 #endif
 KJB_KERNEL_OCC(128, KJB_OCC_RTR_TRACE) k_rtr_trace(const __grid_constant__ Globals g, RtrTraceImgs t, BlueNoiseSamplerTables bn, float4 gts, uint32_t reuse_rtdgi_rays, IrcacheBufs ircache, Rows kjb_rows) {
     KJB_PX; if (x >= t.out0_tex.w || y >= t.out0_tex.h) return;
@@ -225,7 +225,7 @@ KJB_DEV void rtr_validate_quad(const Globals& g, const RtrValidateImgs& t, float
     }
 }
 #ifndef KJB_OCC_RTR_VALIDATE
-#define KJB_OCC_RTR_VALIDATE 8   /* 183 -> 163 us */
+#define KJB_OCC_RTR_VALIDATE 8
 #endif
 KJB_KERNEL_OCC(128, KJB_OCC_RTR_VALIDATE) k_rtr_validate(const __grid_constant__ Globals g, RtrValidateImgs t, float4 gts, IrcacheBufs ircache, int QW, int QH, Rows kjb_rows) {
     KJB_PX; if (x >= QW || y >= QH) return;
@@ -270,7 +270,7 @@ KJB_DEV void find_best_reprojection_in_neighborhood(const Globals& g, const RtrR
     }
 }
 #ifndef KJB_OCC_RTR_RESTIR_TEMPORAL
-#define KJB_OCC_RTR_RESTIR_TEMPORAL 4   /* 107 -> 64 registers: 95 (1 block) -> 81 (3) -> 77 us (4) at 1080p (profiles/r02m_variants.txt, r02n_variants.txt) */
+#define KJB_OCC_RTR_RESTIR_TEMPORAL 4   /* 107 -> 64 registers */
 #endif
 KJB_KERNEL_OCC(256, KJB_OCC_RTR_RESTIR_TEMPORAL) k_rtr_restir_temporal(const __grid_constant__ Globals g, RtrRestirTemporalImgs t, float4 gts, Rows kjb_rows) {
     KJB_PX; if (x >= t.irradiance_out_tex.w || y >= t.irradiance_out_tex.h) return;
@@ -410,7 +410,7 @@ KJB_KERNEL_OCC(256, KJB_OCC_RTR_RESTIR_TEMPORAL) k_rtr_restir_temporal(const __g
 // ------------------------------------------------------------------ R4 resolve.hlsl:78-663 (USE_RESTIR, BORROW_SAMPLES, CUT_CORNERS_IN_MATH)
 struct RtrResolveImgs { Img gbuffer_tex, depth_tex, hit1_tex, reprojection_tex, half_view_normal_tex, ray_len_history_tex, restir_irradiance_tex, restir_ray_tex, restir_reservoir_tex, restir_ray_orig_tex; ImgW output_tex, ray_len_output_tex; };
 #ifndef KJB_OCC_RTR_RESOLVE
-#define KJB_OCC_RTR_RESOLVE 4   /* 98 -> 64 registers (80 B of spills), 4 blocks per SM: 1034 (2 blocks) -> 828 (3) -> 787 us (4) at 1080p (profiles/r02i_variants.txt, r02j_variants.txt) */
+#define KJB_OCC_RTR_RESOLVE 4   /* 98 -> 64 registers, 4 blocks per SM */
 #endif
 // sin / cos of the tap angles `(sample_i + ang_offset) * GOLDEN_ANGLE + (px_idx_in_quad / 4) * TAU`: 4 quad slots x 8 taps = 32 distinct angles per FRAME
 // (ang_offset depends on the frame index only), so the host evaluates them once with the contract's kjb_sincos and every pixel looks its eight up
@@ -740,6 +740,7 @@ static int check_ircache_bindings(kjb_context* c, const char* P, const kjb_ircac
         && b.reposition_proposal_count_buf.data && b.reposition_proposal_count_buf.size_bytes >= 4 * E;
     if (!ok) return c->fail(std::string(P) + ": irradiance cache bindings are incomplete or too small");
     out = ircache_bufs(b);
+    ircache_attach_parallel(c, out);
     return 0;
 }
 

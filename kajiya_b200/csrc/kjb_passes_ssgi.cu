@@ -1,4 +1,4 @@
-// Screen-space ambient occlusion guide (SURVEY §8f N3) as sm_100a kernels — the four passes of
+// Screen-space ambient occlusion guide (SURVEY §8f N3) as sm_90a kernels — the four passes of
 // crates/lib/kajiya/src/renderers/ssgi.rs, shader sources under /root/reference/assets/shaders/ssgi/ (USE_AO_ONLY 1: the shader's
 // lighting gather only feeds an accumulator the AO-only output never reads, so it is not evaluated).
 #include "kjb_context.h"

@@ -1,4 +1,4 @@
-// Temporal anti-aliasing / temporal super-resolution as sm_100a kernels — one per render-graph pass of
+// Temporal anti-aliasing / temporal super-resolution as sm_90a kernels — one per render-graph pass of
 // crates/lib/kajiya/src/renderers/taa.rs:41-185 (shaders: /root/reference/assets/shaders/taa/, inc/unjitter_taa.hlsl, inc/image.hlsl).
 // All seven passes are small-stencil screen-space filters: 32x8 thread blocks on the pass's grid, 8-byte RGBA16F texels =>
 // 256 B per warp-row request; constant filter weights (exp(-r^2 ...)) are evaluated once on the host with the numeric

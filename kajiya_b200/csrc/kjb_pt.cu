@@ -1,4 +1,4 @@
-// "reference pt": kajiya's reference path tracer (rt/reference_path_trace.rgen.hlsl:75-377) as an sm_100a kernel.
+// "reference pt": kajiya's reference path tracer (rt/reference_path_trace.rgen.hlsl:75-377) as an sm_90a kernel.
 // In the reference this IS a GPU pass (renderers/reference.rs:8-25); it doubles as the converged-image yardstick for rtdgi.
 #include "kjb_context.h"
 

@@ -1,4 +1,4 @@
-// Ray traversal + hit shading for B200 SMs.
+// Ray traversal + hit shading for H100 SMs.
 //
 // The reference delegates traversal to VK_KHR_ray_tracing (TraceRay in inc/rt.hlsl:58-70,112-137) and shades hits in
 // rt/gbuffer.rchit.hlsl:46-202.  Here both run in the calling kernel: a stack-based while-while BVH2 walk over 64-byte

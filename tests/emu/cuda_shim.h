@@ -4,7 +4,7 @@
 // (g++ -x c++ -include cuda_shim.h -DKJB_EMU) in front of the unmodified .cu sources, supplies the handful of
 // CUDA built-ins they use (vector types, threadIdx/blockIdx, dim3) and runs every launch as nested loops over
 // blocks and threads (OpenMP over blocks).  The resulting libkjb_emu.so is loaded ONLY by tests/ ("emu-cpu" backend);
-// the product package never builds, loads or falls back to it — kajiya_b200.lib() refuses anything but "cuda-sm100a".
+// the product package never builds, loads or falls back to it — kajiya_b200.lib() refuses anything but "cuda-sm90a".
 #pragma once
 #include <cstdint>
 #include <cstdlib>

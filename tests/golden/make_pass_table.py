@@ -1,15 +1,16 @@
 """Extracts the render-graph pass declarations of the hot path from kajiya's Rust sources — mechanically, so that the table is independent
-of this repo's C++ host mirror — into tests/golden/pass_table.json.  Run in the container that has /root/reference:
+of this repo's C++ host mirror — into tests/golden/pass_table.json.  Run against a checkout of kajiya:
 
-    python tests/golden/make_pass_table.py [/root/reference]
+    python tests/golden/make_pass_table.py <path to the kajiya checkout>
 
 For every `SimpleRenderPass::new_compute / new_rt(rg.add_pass("label"), shader...)` builder chain the table records, in call order, the
 binding methods (`read`, `read_aspect`, `write`, `write_no_sync`, `constants`, `bind`, `bind_mut`, `raw_descriptor_set`, ...) with their
 argument text, and the terminal call (`dispatch`, `dispatch_indirect`, `trace_rays`, `trace_rays_indirect`).  Binding index = call order
-(crates/lib/kajiya-rg/src/hl.rs:266,324,354-359).  tests/test_host_mirror.py asserts kjb_world.cpp against it."""
+(crates/lib/kajiya-rg/src/hl.rs:266,324,354-359).  It also records the order in which the irradiance cache's `bind_mut` binds its buffers.
+tests/test_host_mirror.py asserts kjb_world.cpp against it."""
 import json, os, re, sys
 
-REF = sys.argv[1] if len(sys.argv) > 1 else "/root/reference"
+REF = sys.argv[1]
 FILES = ["crates/lib/kajiya/src/renderers/rtdgi.rs", "crates/lib/kajiya/src/renderers/ircache.rs", "crates/lib/kajiya/src/renderers/rtr.rs",
          "crates/lib/kajiya/src/renderers/taa.rs", "crates/lib/kajiya/src/renderers/reprojection.rs", "crates/lib/kajiya/src/renderers/half_res.rs",
          "crates/lib/kajiya/src/renderers/ssgi.rs", "crates/lib/kajiya/src/renderers/lighting.rs", "crates/lib/kajiya/src/renderers/shadow_denoise.rs",
@@ -70,12 +71,21 @@ def passes_of(path):
     return out
 
 
+def ircache_bind_mut_order():
+    """buffer fields in the order `BindMutToSimpleRenderPass for IrcacheRenderState` (ircache.rs) binds them"""
+    src = open(os.path.join(REF, "crates/lib/kajiya/src/renderers/ircache.rs")).read()
+    body = src[src.index("impl<'rg, RgPipelineHandle> BindMutToSimpleRenderPass"):]
+    body = body[:body.index("\n}\n")]
+    return re.findall(r"(?:write_no_sync|read)\(&(?:mut )?self\.(\w+)\)", body)
+
+
 table = []
 for f in FILES:
     if os.path.exists(os.path.join(REF, f)):
         table += passes_of(f)
 dst = os.path.join(os.path.dirname(os.path.abspath(__file__)), "pass_table.json")
-json.dump({"source": "EmbarkStudios/kajiya @ 9fdec0f, crates/lib/kajiya/src/renderers/*.rs", "generator": "tests/golden/make_pass_table.py", "passes": table}, open(dst, "w"), indent=1)
+json.dump({"source": "EmbarkStudios/kajiya @ 9fdec0f, crates/lib/kajiya/src/renderers/*.rs", "generator": "tests/golden/make_pass_table.py", "passes": table,
+           "ircache_bind_mut_order": ircache_bind_mut_order()}, open(dst, "w"), indent=1)
 print(len(table), "passes ->", dst)
 for p in table:
     print(f'{p["file"].split("/")[-1]}:{p["line"]:<4} {p["label"] or p["label_expr"]!s:32} {len(p["calls"]):2} calls  {p["terminal"]["m"] if p["terminal"] else "?"}')

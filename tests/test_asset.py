@@ -1,6 +1,6 @@
 """Asset import (SURVEY §8 row N5): libkjb_asset.so (C++: glTF 2.0 -> TriangleMesh, PNG / JPEG -> RGBA8, Lanczos3 mip chains) against the
 numpy restatement oracle/kj_asset.py, committed fixtures (tests/golden/gltf, made by tests/golden/make_gltf_fixtures.py), hand-computed
-expectations, and — in this container only — the reference's own bundled glTF assets.  Bit-exact everywhere except JPEG (lossy codec:
+expectations, and the reference's own bundled glTF assets (the small ones, stored under tests/golden/reference_assets).  Bit-exact everywhere except JPEG (lossy codec:
 max / mean texel error against libjpeg stated in the test)."""
 import ctypes as C, glob, io, json, os, re, sys, zlib
 import numpy as np, pytest
@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.join(conftest.ROOT, "oracle"))
 import kj_asset as oracle   # noqa: E402  (test infrastructure)
 
 FIX = os.path.join(conftest.ROOT, "tests", "golden", "gltf")
-REF_MESHES = "/root/reference/assets/meshes"
+REF_MESHES = os.path.join(conftest.ROOT, "tests", "golden", "reference_assets", "meshes")
 
 
 def bits(a):
@@ -321,20 +321,18 @@ def test_json_parser_corner_cases(tmp_path):
             asset.GltfScene(str(q))
 
 
-# ------------------------------------------------------------------ the reference's own bundled assets (this container only)
-REF_CASES = [("cornell_box/scene.gltf", 0), ("floor/scene.gltf", 0), ("roughness-scale/scene.gltf", 0), ("emissive/triangle.glb", 0), ("336_lrm/scene.gltf", 0),
-             ("conference/scene.gltf", 8)]
+# ------------------------------------------------------------------ the reference's own bundled assets
+REF_CASES = [("cornell_box/scene.gltf", 0), ("floor/scene.gltf", 0), ("roughness-scale/scene.gltf", 0), ("emissive/triangle.glb", 0),
+             ("conference_jake/scene.gltf", 8)]   # the textured node of the reference's conference scene (tests/golden/make_reference_subsets.py)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MESHES), reason="reference assets are only present in the build container")
 @pytest.mark.parametrize("rel,texel_tol", REF_CASES, ids=[c[0].split("/")[0] for c in REF_CASES])
 def test_reference_assets_match_the_restatement(rel, texel_tol):
-    """conference/ carries a JPEG: its maps are compared within 8/255 (decoder + resampling of decoder differences), everything else exactly"""
+    """conference_jake carries a JPEG: its maps are compared within 8/255 (decoder + resampling of decoder differences), everything else exactly"""
     path = os.path.join(REF_MESHES, rel)
     assert_same_mesh(asset.GltfScene(path).arrays(), oracle.load_gltf_scene(path), texel_tol)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_MESHES), reason="reference assets are only present in the build container")
 def test_bundled_cornell_box_fixture_is_the_reference_asset():
     """kajiya_b200/assets/cornell_box.json (the bench scene, baked in float64 by tests/golden/make_assets.py) is the same mesh the importer
     produces from the reference's scene.gltf: identical topology and materials, vertices within one float32 ulp of the f32 transform chain."""

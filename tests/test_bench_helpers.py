@@ -1,4 +1,4 @@
-"""bench.py pieces that can be checked without a GPU (the driver runs the script itself on the B200)."""
+"""bench.py pieces that can be checked without a GPU."""
 import importlib.util, os
 import conftest
 
@@ -58,3 +58,19 @@ def test_band_compare():
     ok, exact, *_ = b.band_compare(a, t, 64, 1, 4, False)
     assert not ok and not exact
     assert b.band_compare(a, t, 64, 1, 4, True)[0]                   # statistical mode tolerates it
+
+
+def test_dump_outputs_writes_float32_within_the_budget(tmp_path):
+    b = _bench()
+    import numpy as np
+    b.DUMP_BYTES = 1 << 20
+    small = np.arange(24, dtype=np.float16).reshape(2, 3, 4)
+    big = np.random.RandomState(2).rand(512, 256, 4).astype(np.float16)   # 2 MiB as float32: over the budget
+    b.dump_outputs(str(tmp_path / "a"), {"small": small, "big": big})
+    b.dump_outputs(str(tmp_path / "b"), {"small": small, "big": big})
+    s, g = np.load(tmp_path / "a" / "small.npy"), np.load(tmp_path / "a" / "big.npy")
+    assert s.dtype == np.float32 and np.array_equal(s, small.astype(np.float32))
+    assert g.dtype == np.float32 and g.shape[1:] == big.shape[1:] and 0 < g.shape[0] < big.shape[0]
+    assert sum(os.path.getsize(p) for p in (tmp_path / "a").iterdir()) <= b.DUMP_BYTES
+    assert np.array_equal(g, np.load(tmp_path / "b" / "big.npy"))     # the sample is fixed
+    assert all(any(np.array_equal(r, x) for x in big.astype(np.float32)) for r in g[:8])

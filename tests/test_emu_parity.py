@@ -337,3 +337,66 @@ def test_shadow_denoiser_neighbourhood_against_a_plain_convolution(oracle_lib):
     # cleared tiles carry the uniform value instead
     cleared_lit = np.kron(meta == 3, np.ones((8, 8), bool))[:h_, :w_]
     assert (got[cleared_lit] == 1.0).all()
+
+
+ORDERED_CACHE_SCHEDULE = 2   # KJB_OPTION_ORDERED_CACHE_SCHEDULE (kjb.h): the GPU's default, off in the emulator unless set
+
+
+def _ordered_cache_invariants(w):
+    """the bookkeeping of the ordered schedule: live entries = the allocated count, one entry per cell, every other entry free (none
+    leaked), and no live entry at or beyond entry_count.  (The pool is rebuilt from the free entries at the start of each chain.)"""
+    meta = w.image("ircache.meta_buf").ravel()
+    life = w.image("ircache.life_buf").ravel()
+    cell = w.image("ircache.entry_cell_buf").ravel()
+    live = np.nonzero(life < 12)[0]
+    assert int(meta[3]) == len(live), (int(meta[3]), len(live))
+    assert len(set(cell[live].tolist())) == len(live)
+    assert len(live) == 0 or int(live.max()) < int(meta[2])
+    assert int((life == 0x8000001).sum()) + len(live) == len(life)
+
+
+def test_ordered_cache_schedule_against_the_oracle(oracle_lib, emu_lib):
+    """The GPU's default cache schedule (kjb_ircache.cuh) run by the emulator: claims wait for the next chain and take entries in cell
+    order, keep-alives wait too, votes go to the smallest hash.  Under a moving camera (scrolling, deallocation, ageing, recycling) its
+    bookkeeping stays consistent every frame; on a still camera it settles where the oracle's schedule does (live entries within 5 %,
+    mean L0 irradiance of the live entries and of the GI image within 10 %)."""
+    scene, view = scenes.cornell_box()
+    kw = dict(enable_ircache=True, spatial_reuse_pass_count=1)
+    w = parity.make_world(emu_lib, scene, 80, 48, **kw)
+    w.set_option(ORDERED_CACHE_SCHEDULE, 1)
+    peak = 0
+    for v in _moving_views(view, 16):
+        w.render_frame(**v)
+        _ordered_cache_invariants(w)
+        peak = max(peak, int(w.image("ircache.meta_buf").ravel()[3]))
+    assert 0 < int(w.image("ircache.meta_buf").ravel()[3]) < peak         # entries were allocated and recycled
+
+    wa, wb = parity.make_world(oracle_lib, scene, 96, 64, **kw), parity.make_world(emu_lib, scene, 96, 64, **kw)
+    wb.set_option(ORDERED_CACHE_SCHEDULE, 1)
+    for f in range(12):
+        wa.render_frame(**view); wb.render_frame(**view)
+    _ordered_cache_invariants(wb)
+    def summary(x):
+        life = x.image("ircache.life_buf").ravel()
+        irr = x.image("ircache.irradiance_buf").reshape(-1, 3, 4)
+        return int(x.image("ircache.meta_buf").ravel()[3]), float(irr[life < 12][:, :, 0].mean()), float(x.image("rtdgi.spatial_filtered").astype(np.float64)[..., :3].mean())
+    (na, ra, ga), (nb, rb, gb) = summary(wa), summary(wb)
+    assert abs(na - nb) <= 0.05 * na + 2, (na, nb)
+    assert abs(ra - rb) <= 0.10 * abs(ra), (ra, rb)
+    assert abs(ga - gb) <= 0.10 * ga, (ga, gb)
+
+
+def test_cache_schedule_cannot_change_under_pending_claims(emu_lib):
+    """the ordered schedule keeps claims pending until the next chain: switching to another schedule after it ran is refused"""
+    import pytest
+    from kajiya_b200._abi import KjbError
+    scene, view = scenes.cornell_box()
+    w = parity.make_world(emu_lib, scene, 48, 32, enable_ircache=True)
+    w.set_option(ORDERED_CACHE_SCHEDULE, 1)
+    w.render_frame(**view)
+    with pytest.raises(KjbError):
+        w.set_debug_serial(True)
+    with pytest.raises(KjbError):
+        w.set_option(ORDERED_CACHE_SCHEDULE, 0)
+    w.render_frame(**view)
+    _ordered_cache_invariants(w)

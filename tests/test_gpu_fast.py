@@ -21,7 +21,7 @@ def _rel_l2(a, b):
 
 
 def test_fast_build_is_a_different_backend(fast_lib, cuda_lib):
-    assert fast_lib.backend == "cuda-sm100a-fast" and cuda_lib.backend == "cuda-sm100a"
+    assert fast_lib.backend == "cuda-sm90a-fast" and cuda_lib.backend == "cuda-sm90a"
 
 
 def test_first_frame_tier_b(fast_lib, cuda_lib):

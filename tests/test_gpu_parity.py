@@ -13,7 +13,7 @@ def _assert_clean(report):
 
 
 def test_backend_is_cuda(cuda_lib):
-    assert cuda_lib.backend == "cuda-sm100a"
+    assert cuda_lib.backend == "cuda-sm90a"
 
 
 def test_cornell_rtdgi_lockstep(oracle_lib, cuda_lib):
@@ -87,8 +87,8 @@ def _moving_views(view, frames):
 
 
 def test_ircache_serial_schedule_bit_exact(oracle_lib, cuda_lib):
-    """The irradiance cache is racy by design (ircache.rs:68-76), so its state depends on GPU scheduling.  With
-    kjb_set_debug_serial the CUDA kernels that touch the cache run on one device thread in launch order — the schedule the
+    """The irradiance cache is racy by design upstream (ircache.rs:68-76); the default parallel schedule decides differently from the
+    oracle's (kjb_ircache.cuh).  With kjb_set_debug_serial the CUDA kernels that touch the cache run on one device thread in launch order — the schedule the
     oracle restates — and then EVERYTHING (images + grid/pool/reservoir/SH buffers) must be bit-identical, including cascade
     scrolling, deallocation, aging and recycling under a moving camera."""
     scene, view = scenes.cornell_box()
@@ -112,8 +112,8 @@ def _cache_summary(w):
 
 
 def test_ircache_parallel_statistical(oracle_lib, cuda_lib):
-    """Normal (parallel, racy) execution against the oracle's serial schedule: which thread wins an allocation or a reposition
-    vote differs, so parity is statistical.  Tolerances: live entry count 3 %, occupied-cell sets Jaccard >= 0.9 (either buffer
+    """Normal (parallel) execution against the oracle's serial schedule: entry assignment, keep-alive and reposition votes are decided
+    differently (kjb_ircache.cuh), so parity is statistical.  Tolerances: live entry count 3 %, occupied-cell sets Jaccard >= 0.9 (either buffer
     parity), mean L0 irradiance over the live entries 12 % (a few hundred entries after 12 frames: observed spread between GPU runs ~6 %), mean of the final GI image 6 % (observed up to 3 % between racy runs), and the final image within 0.05 RMS of the oracle's."""
     scene, view = scenes.cornell_box()
     kw = dict(enable_ircache=True)
@@ -286,9 +286,9 @@ def test_atrium_full_path_serial_schedule_480x270(oracle_lib, cuda_lib):
 
 
 def test_atrium_1080p_full_path_parallel_statistical(oracle_lib, cuda_lib):
-    """BASELINE configs[2] exactly as bench.py times it — atrium 1080p, rtdgi + ircache + rtr + taa, the PARALLEL (racy) cache kernels — against the
-    oracle's serial schedule.  Statistical by necessity (which thread wins an allocation, and whether a pixel sees an entry allocated earlier in
-    the SAME pass, differs): live cache entries within 5 %, mean of the GI / final images within 15 %, per-image RMS difference below 20 % of the
+    """BASELINE configs[2] exactly as bench.py times it — atrium 1080p, rtdgi + ircache + rtr + taa, the PARALLEL cache kernels — against the
+    oracle's serial schedule.  Statistical by necessity (entries are assigned in cell order at the next chain, reposition votes go to the smallest
+    hash, and no pixel sees an entry allocated earlier in the SAME pass): live cache entries within 5 %, mean of the GI / final images within 15 %, per-image RMS difference below 20 % of the
     image mean, mean L0 irradiance of the live entries within 40 % after 8 frames (a few samples per entry: the serial schedule lets late
     pixels of a pass hit entries the early ones just allocated, the parallel one does not)."""
     scene, view = scenes.atrium()
@@ -307,20 +307,33 @@ def test_atrium_1080p_full_path_parallel_statistical(oracle_lib, cuda_lib):
     assert abs(m["r0"][0] - m["r0"][1]) <= 0.30 * abs(m["r0"][0]), m
     for name in ("rtdgi.spatial_filtered", "taa.this_frame_out"):
         ma, mb, rms = m[name]
-        assert abs(ma - mb) <= 0.15 * ma, m     # recorded runs: +3.6 % (profiles/r02m_gpu_tests.txt) ... +9.0 % (r02h): the parallel schedule runs brighter while the cache fills
+        assert abs(ma - mb) <= 0.15 * ma, m     # the parallel schedule runs brighter while the cache fills
         assert rms <= 0.20 * ma, m
     # images that never see the cache are still exact: the G-buffer side and the reprojection map
     assert not parity.compare_images(wa, wb, names=["depth", "gbuffer", "reprojection_map", "half_depth", "half_view_normal"])
 
 
+def test_parallel_cache_schedule_is_deterministic(cuda_lib):
+    """The default (parallel) schedule of the irradiance cache decides independently of the order its threads run in: two worlds rendering the
+    same frames of the full path — cache filling from cold, cells claimed, entries assigned, aged and moved by votes — hold the same bits in every
+    image and buffer, the cache's included."""
+    scene, view = scenes.atrium()
+    kw = dict(enable_rtr=True, enable_ircache=True, enable_taa=True, spatial_reuse_pass_count=2)
+    wa, wb = parity.make_world(cuda_lib, scene, 480, 270, **kw), parity.make_world(cuda_lib, scene, 480, 270, **kw)
+    for f in range(12):
+        wa.render_frame(**view); wb.render_frame(**view)
+        bad = parity.compare_images(wa, wb)
+        assert not bad, (f, bad[:8])
+    assert int(wb.image("ircache.meta_buf").ravel()[3]) > 100
+
+
 def test_async_cache_chain_matches_in_order_submission(cuda_lib):
     """From the fifth frame on the irradiance-cache chain of a frame runs on the async pass queue, under the previous frame's reflection filters + TAA
     (kjb_world_set_async_compute), and the frame is submitted as three graph recordings around the two ordering points.  Against the same frames submitted
-    in program order on one queue: the cache is racy either way, so the comparison is statistical (live entries 4 %, mean L0 irradiance of the live
+    in program order on one queue: the comparison is statistical (live entries 4 %, mean L0 irradiance of the live
     entries 15 %, image means 8 %, RMS difference 20 % of the mean.  The yardstick is the renderer's own run-to-run spread: two in-order single-GPU renders of
-    the same 24 frames differ by up to 4.0 % in the mean of a half-frame band (`parity.untiled_vs_untiled` in profiles/r02w_bench_n2.json); this test's first
-    recorded run had the two images 3.7 % apart, RMS 10 %); the images that never see the cache
-    stay bit-identical."""
+    the same 24 frames differ by a few per cent in the mean of a half-frame band, `parity.untiled_vs_untiled` of a `bench.py --gpus 2` line); the images that
+    never see the cache stay bit-identical."""
     scene, view = scenes.atrium()
     kw = dict(enable_rtr=True, enable_ircache=True, enable_taa=True, spatial_reuse_pass_count=2)
     wa, wb = parity.make_world(cuda_lib, scene, 960, 540, **kw), parity.make_world(cuda_lib, scene, 960, 540, **kw)

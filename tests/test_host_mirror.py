@@ -229,18 +229,9 @@ def frame_sequence(feat, frame, spatial_passes):
     return seq
 
 
-def test_pass_table_fixture_is_current():
-    """the committed fixture is what the generator extracts from the reference (only checkable where /root/reference exists)"""
-    if not os.path.isdir("/root/reference/crates"):
-        pytest.skip("reference sources are not on this machine")
-    before = open(os.path.join(conftest.ROOT, "tests", "golden", "pass_table.json")).read()
-    subprocess.run(["python", os.path.join(conftest.ROOT, "tests", "golden", "make_pass_table.py")], check=True, stdout=subprocess.DEVNULL)
-    assert open(os.path.join(conftest.ROOT, "tests", "golden", "pass_table.json")).read() == before
-    src = open("/root/reference/crates/lib/kajiya/src/renderers/ircache.rs").read()
-    body = src[src.index("impl<'rg, RgPipelineHandle> BindMutToSimpleRenderPass"):]
-    body = body[:body.index("\n}\n")]
-    order = re.findall(r"write_no_sync\(&mut self\.(\w+)\)", body)
-    order = re.findall(r"(?:write_no_sync|read)\(&(?:mut )?self\.(\w+)\)", body)
+def test_ircache_bind_order_matches_the_reference():
+    """the mirror binds the irradiance-cache buffers in the order the reference's `bind_mut` does (extracted into the fixture by make_pass_table.py)"""
+    order = json.load(open(os.path.join(conftest.ROOT, "tests", "golden", "pass_table.json")))["ircache_bind_mut_order"]
     want = [n.split(".")[1] if n != "GRID" else "grid_meta_buf" for n in IRCACHE_BIND_MUT]
     assert [o.replace("ircache_", "") for o in order] == want, order
 

@@ -152,7 +152,7 @@ def test_tile_sharded_reflections_match_single_process(emu_lib):
 
 
 def test_tile_sharded_frames_with_host_inputs(emu_lib):
-    """host G-buffers in, result out, 2 ranks: each rank uploads only its band of the inputs, an all-gather distributes the bands (NVLink on the B200),
+    """host G-buffers in, result out, 2 ranks: each rank uploads only its band of the inputs, an all-gather distributes the bands (NVLink on a multi-GPU box),
     the frame is rendered tile-sharded and each rank hands back its band of the result — bit-identical to the single-process frame"""
     ret = mp.Manager().dict()
     mp.spawn(_worker, args=(2, _free_port(), False, H, ret, False, True), nprocs=2, join=True)

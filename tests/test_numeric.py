@@ -89,11 +89,11 @@ def test_integer_over_constant_division_is_ieee_exact(num):
 
 
 def test_min_max_order_signed_zeros_and_drop_nans(num):
-    """IEEE 754-2019 minimumNumber / maximumNumber — what FMNMX does on sm_100a (tools/probe_minmax.cu)"""
+    """IEEE 754-2019 minimumNumber / maximumNumber — what FMNMX does on sm_90a (tools/probe_minmax.cu)"""
     u = lambda *w: np.array(w, np.uint32).view(np.float32)
     a = u(0x00000000, 0x80000000, 0x00000000, 0x80000000, 0x7fc00000, 0x3f800000, 0xffc12345, 0x80000000, 0x7fc00000, 0x00000001, 0x80000001)
     b = u(0x80000000, 0x00000000, 0x00000000, 0x80000000, 0x3f800000, 0x7fc00000, 0x80000000, 0xffc12345, 0xffc12345, 0x80000001, 0x00000001)
-    mn = u(0x80000000, 0x80000000, 0x00000000, 0x80000000, 0x3f800000, 0x3f800000, 0x80000000, 0x80000000, 0x7fffffff, 0x80000001, 0x80000001)   # as printed by the B200
+    mn = u(0x80000000, 0x80000000, 0x00000000, 0x80000000, 0x3f800000, 0x3f800000, 0x80000000, 0x80000000, 0x7fffffff, 0x80000001, 0x80000001)   # as printed by the H100
     mx = u(0x00000000, 0x00000000, 0x00000000, 0x80000000, 0x3f800000, 0x3f800000, 0x80000000, 0x80000000, 0x7fffffff, 0x00000001, 0x00000001)
     assert np.array_equal(_call(num, "t_min", a, b).view(np.uint32), mn.view(np.uint32))
     assert np.array_equal(_call(num, "t_max", a, b).view(np.uint32), mx.view(np.uint32))

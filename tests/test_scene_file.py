@@ -6,7 +6,8 @@ from kajiya_b200 import scene_file, scenes
 from kajiya_b200.world import World
 
 GOLDEN = os.path.join(conftest.ROOT, "tests", "golden")
-REF_SCENES = "/root/reference/assets/scenes"
+REF_ASSETS = os.path.join(GOLDEN, "reference_assets")   # the reference's scene files and the meshes the Cornell box scene names
+REF_SCENES = os.path.join(REF_ASSETS, "scenes")
 
 
 def test_parse_fixture_and_defaults():
@@ -53,7 +54,6 @@ def test_load_scene_on_a_world(oracle_lib, emu_lib):
     assert (worlds[1].image("depth") > 0).mean() > 0.1
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_SCENES), reason="reference scene files are only present in the build container")
 def test_reference_scene_files_parse():
     files = sorted(glob.glob(os.path.join(REF_SCENES, "*.ron")))
     assert len(files) >= 9
@@ -65,12 +65,11 @@ def test_reference_scene_files_parse():
                                                                               np.array([[2, 0, 0, 0], [0, 2, 0, -1], [0, 0, 2, 0]], np.float32))
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_SCENES), reason="reference assets are only present in the build container")
 def test_reference_cornell_scene_loads_like_the_bundled_one(emu_lib):
     """cornell_box.ron through scene_file + the glTF importer gives the geometry of kajiya_b200.scenes.cornell_box() (the bench scene):
     same depth buffer to within the 1-ulp vertex difference documented in test_asset.py"""
     import parity
-    wa = World(emu_lib, 64, 64); scene_file.load_scene(wa, os.path.join(REF_SCENES, "cornell_box.ron"), "/root/reference/assets"); wa.set_blue_noise(scenes.blue_noise())
+    wa = World(emu_lib, 64, 64); scene_file.load_scene(wa, os.path.join(REF_SCENES, "cornell_box.ron"), REF_ASSETS); wa.set_blue_noise(scenes.blue_noise())
     scene, view = scenes.cornell_box(); wb = parity.make_world(emu_lib, scene, 64, 64)
     wa.render_frame(**view); wb.render_frame(**view)
     da, db = wa.image("depth")[..., 0], wb.image("depth")[..., 0]

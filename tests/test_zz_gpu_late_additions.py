@@ -1,6 +1,5 @@
-"""GPU twins of features that were written after this round's GPU budget was spent (their CPU-emulator versions are in test_emu_parity.py /
-test_multigpu_gloo.py and are bit-exact against the oracle).  The file sorts last on purpose: the first time these run on a B200 is the
-driver's round-end `pytest -m gpu`, after every test that has already been green on the hardware."""
+"""GPU twins of features whose CPU-emulator versions are in test_emu_parity.py / test_multigpu_gloo.py (bit-exact against the oracle).
+The file sorts last on purpose: a `pytest -m gpu` run reaches it after every older GPU test."""
 import os
 import numpy as np, pytest
 import conftest, parity

@@ -1,5 +1,5 @@
 """Markdown table for DESIGN.md §5e: every pass of the headline frame with its algorithmic bytes (bench.PASS_BYTES, SURVEY §8a), its measured time (a bench line),
-the HBM roofline fraction that follows, and what ncu says bounds it (profiles/ncu_kernel_table.json).   python tools/kernel_table.py profiles/<bench>.json"""
+the HBM roofline fraction that follows, and what ncu says bounds it (profiles/ncu_kernel_table.json, where present).   python tools/kernel_table.py <bench line>.json"""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import bench
@@ -7,7 +7,7 @@ b = json.loads(open(sys.argv[1]).read().strip().splitlines()[-1])
 wl = b["config"]["workload"]; W, H = b["config"]["resolution"]; OW, OH = b["config"]["output_resolution"]
 F, Hh, O = W * H, ((W + 1) // 2) * ((H + 1) // 2), OW * OH
 peak = b["roofline"]["peak"]; pp = b["roofline"]["per_pass_ms"]
-ncu = json.load(open(os.path.join(ROOT, "profiles", "ncu_kernel_table.json"))).get(wl, {})
+ncu = bench.load_ncu_table().get(wl, {})
 print("| pass (rg label) | algorithmic bytes | per launch | ms | GB/s | % of HBM peak | ncu DRAM MB | issue-active % | occupancy % | lanes / inst | bound by |")
 print("|---|---|---|---|---|---|---|---|---|---|---|")
 for k, ms in sorted(pp.items(), key=lambda kv: -kv[1]):

@@ -3,7 +3,7 @@ barriers (SYNCS.*) and warp shuffles (SHFL.*) — from `cuobjdump -sass` of the 
 import subprocess, re, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 objs = ['kjb_passes_taa.cu.o', 'kjb_passes_rtdgi.cu.o', 'kjb_passes_rtr.cu.o', 'kjb_passes_ircache.cu.o', 'kjb_api.cu.o']
-out = ["# SASS evidence (cuobjdump -sass of kajiya_b200/csrc/_obj/*.o, sm_100a, the shipping build): TMA-engine copies (UBLKCP = cp.async.bulk, UTMALDG = cp.async.bulk.tensor),",
+out = ["# SASS evidence (cuobjdump -sass of kajiya_b200/csrc/_obj/*.o, sm_90a, the shipping build): TMA-engine copies (UBLKCP = cp.async.bulk, UTMALDG = cp.async.bulk.tensor),",
        "# transaction barriers (SYNCS.*), warp shuffles (SHFL.*) per kernel: instruction counts and one line per distinct form.  Regenerate: python tools/sass_excerpts.py", ""]
 pat = re.compile(r'UBLKCP|UTMALDG|SYNCS\.|SHFL\.|ELECT')
 for o in objs:

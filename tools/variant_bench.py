@@ -25,7 +25,7 @@ def build(specs):
             cmd = [g.NVCC] + [f for f in g.NVCC_FLAGS if f not in ("-Xptxas", "-v")] + flags + ["-x", "cu" if src.endswith(".cu") else "c++", "-c", os.path.join(g.CSRC, src), "-o", obj]
             procs.append(subprocess.Popen(cmd))
         assert all(p.wait() == 0 for p in procs)
-        subprocess.check_call([g.NVCC, "-shared", "-o", os.path.join(VAR, f"libkjb_{name}.so")] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"])
+        subprocess.check_call([g.NVCC, "-shared", "-o", os.path.join(VAR, f"libkjb_{name}.so")] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"])
         for o in objs: os.remove(o)
         print("built", name, flags)
 
