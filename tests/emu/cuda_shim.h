@@ -3,7 +3,7 @@
 // There is no GPU in the build container, so kernel LOGIC is debugged here: this header is force-included
 // (g++ -x c++ -include cuda_shim.h -DKJB_EMU) in front of the unmodified .cu sources, supplies the handful of
 // CUDA built-ins they use (vector types, threadIdx/blockIdx, dim3) and runs every launch as nested loops over
-// blocks and threads (OpenMP over blocks).  The resulting libkjb_emu.so is loaded ONLY by tests/ ("emu-cpu" backend);
+// blocks and threads (blocks spread over worker threads).  The resulting libkjb_emu.so is loaded ONLY by tests/ ("emu-cpu" backend);
 // the product package never builds, loads or falls back to it — kajiya_b200.lib() refuses anything but "cuda-sm90a".
 #pragma once
 #include <cstdint>
@@ -42,18 +42,36 @@ extern thread_local dim3 blockDim, gridDim;
 namespace kjb_emu {
 int num_workers();
 extern int g_serial;   // > 0: run blocks one after another in launch order (KJB_LAUNCH_ORDERED)
+
+// Launch order (kjb_emu_set_launch_order): 0 = forward, 1 = reverse, 2 = a seeded permutation per launch.  The k-th block (thread) a
+// launch runs is `order.at(k)`: the bijection k -> (a * k + c) mod n with gcd(a, n) = 1, so nothing is allocated per launch.  Kernels
+// whose result may depend on the order their threads run in are bugs on the GPU; running them in another order here shows them.
+struct Order {
+    uint64_t a = 1, c = 0, n = 1;
+    long at(long k) const { return long((a * uint64_t(k) + c) % n); }
+};
+Order launch_order(uint64_t n, uint64_t key);   // key: which launch / block / barrier phase (mode 2 mixes it into the seed)
+uint64_t next_launch_key();
+// runs worker(0) .. worker(n - 1) concurrently, worker(0) on the calling thread.  The other workers are threads that persist across launches:
+// a thread per launch would pay thread creation, a fresh TLS block (every kernel's __shared__ arrays) and fresh fiber stacks every time.
+void run_workers(int n, void (*worker)(void*), void* arg);
 template <typename F> inline void launch(dim3 grid, dim3 block, F body) {
     const long nblocks = long(grid.x) * grid.y * grid.z;
+    const unsigned nthreads = block.x * block.y * block.z;
+    const uint64_t key = next_launch_key();
+    const Order bo = launch_order(uint64_t(nblocks), key * 2), to = launch_order(nthreads, key * 2 + 1);
     std::atomic<long> next{0};
     auto worker = [&]() {
         for (;;) {
             const long b0 = next.fetch_add(4);
             if (b0 >= nblocks) break;
-            for (long b = b0; b < b0 + 4 && b < nblocks; ++b) {
+            for (long k = b0; k < b0 + 4 && k < nblocks; ++k) {
+                const long b = bo.at(k);
                 gridDim = grid; blockDim = block;
                 blockIdx.x = unsigned(b % grid.x); blockIdx.y = unsigned((b / grid.x) % grid.y); blockIdx.z = unsigned(b / (long(grid.x) * grid.y));
-                for (unsigned tz = 0; tz < block.z; ++tz) for (unsigned ty = 0; ty < block.y; ++ty) for (unsigned tx = 0; tx < block.x; ++tx) {
-                    threadIdx.x = tx; threadIdx.y = ty; threadIdx.z = tz;
+                for (unsigned j = 0; j < nthreads; ++j) {
+                    const unsigned t = unsigned(to.at(j));
+                    threadIdx.x = t % block.x; threadIdx.y = (t / block.x) % block.y; threadIdx.z = t / (block.x * block.y);
                     body();
                 }
             }
@@ -61,31 +79,30 @@ template <typename F> inline void launch(dim3 grid, dim3 block, F body) {
     };
     const int n = (nblocks < 16 || g_serial > 0) ? 1 : num_workers();
     if (n <= 1) { worker(); return; }
-    std::vector<std::thread> th;
-    for (int i = 0; i < n; ++i) th.emplace_back(worker);
-    for (auto& t : th) t.join();
+    run_workers(n, [](void* w) { (*static_cast<decltype(worker)*>(w))(); }, &worker);
 }
 // Kernels that use __syncthreads(): every thread of a block runs as a ucontext fiber; a barrier yields to the block
-// scheduler, which resumes each unfinished fiber once per barrier phase.
-void fiber_run_block(unsigned nthreads, dim3 block, void (*thread_body)(void*), void* arg);
+// scheduler, which resumes each unfinished fiber once per barrier phase (in the launch order's sequence; `key` picks the phase's permutation).
+void fiber_run_block(unsigned nthreads, dim3 block, void (*thread_body)(void*), void* arg, uint64_t key);
 void fiber_barrier();
 template <typename F> inline void launch_sync(dim3 grid, dim3 block, F body) {
     const long nblocks = long(grid.x) * grid.y * grid.z;
+    const uint64_t key = next_launch_key();
+    const Order bo = launch_order(uint64_t(nblocks), key * 2);
     std::atomic<long> next{0};
     auto worker = [&]() {
         for (;;) {
-            const long b = next.fetch_add(1);
-            if (b >= nblocks) break;
+            const long k = next.fetch_add(1);
+            if (k >= nblocks) break;
+            const long b = bo.at(k);
             gridDim = grid; blockDim = block;
             blockIdx.x = unsigned(b % grid.x); blockIdx.y = unsigned((b / grid.x) % grid.y); blockIdx.z = unsigned(b / (long(grid.x) * grid.y));
-            fiber_run_block(block.x * block.y * block.z, block, [](void* p) { (*static_cast<F*>(p))(); }, &body);
+            fiber_run_block(block.x * block.y * block.z, block, [](void* p) { (*static_cast<F*>(p))(); }, &body, (key << 24) ^ uint64_t(b));
         }
     };
     const int n = nblocks < 4 ? 1 : num_workers();
     if (n <= 1) { worker(); return; }
-    std::vector<std::thread> th;
-    for (int i = 0; i < n; ++i) th.emplace_back(worker);
-    for (auto& t : th) t.join();
+    run_workers(n, [](void* w) { (*static_cast<decltype(worker)*>(w))(); }, &worker);
 }
 }  // namespace kjb_emu
 inline void __syncthreads() { kjb_emu::fiber_barrier(); }

@@ -259,7 +259,7 @@ def test_cornell_1080p_lockstep_config2(oracle_lib, cuda_lib):
 
 
 def test_atrium_1080p_rtdgi_rtr_taa_lockstep(oracle_lib, cuda_lib):
-    """BASELINE configs[2]'s scene and size without the (racy) cache: the 260 k-triangle atrium at 1920x1080, rtdgi with two spatial passes +
+    """BASELINE configs[2]'s scene and size without the cache (whose ordered schedule the oracle does not restate): the 260 k-triangle atrium at 1920x1080, rtdgi with two spatial passes +
     reflections + TAA, camera in motion — the parallel production kernels of every pass but the cache's, every image bit for bit."""
     scene, view = scenes.atrium()
     kw = dict(enable_rtr=True, enable_taa=True, spatial_reuse_pass_count=2)
@@ -329,33 +329,22 @@ def test_parallel_cache_schedule_is_deterministic(cuda_lib):
 
 def test_async_cache_chain_matches_in_order_submission(cuda_lib):
     """From the fifth frame on the irradiance-cache chain of a frame runs on the async pass queue, under the previous frame's reflection filters + TAA
-    (kjb_world_set_async_compute), and the frame is submitted as three graph recordings around the two ordering points.  Against the same frames submitted
-    in program order on one queue: the comparison is statistical (live entries 4 %, mean L0 irradiance of the live
-    entries 15 %, image means 8 %, RMS difference 20 % of the mean.  The yardstick is the renderer's own run-to-run spread: two in-order single-GPU renders of
-    the same 24 frames differ by a few per cent in the mean of a half-frame band, `parity.untiled_vs_untiled` of a `bench.py --gpus 2` line); the images that
-    never see the cache stay bit-identical."""
+    (kjb_world_set_async_compute), and the frame is submitted as three graph recordings around the two ordering points.  The cache's ordered schedule
+    makes the same decisions whatever the order its threads run in, so against the same frames submitted in program order on one queue every image
+    and cache buffer is bit-identical after every frame; a difference means a missing dependency between the queues."""
     scene, view = scenes.atrium()
     kw = dict(enable_rtr=True, enable_ircache=True, enable_taa=True, spatial_reuse_pass_count=2)
     wa, wb = parity.make_world(cuda_lib, scene, 960, 540, **kw), parity.make_world(cuda_lib, scene, 960, 540, **kw)
     wb.set_async_compute(False)
     for f in range(16):
         wa.render_frame(**view); wb.render_frame(**view)
+        bad = parity.compare_images(wa, wb)
+        assert not bad, (f, bad[:8])
     ga, gb = wa.graph_stats(), wb.graph_stats()
     assert ga["launches"] == 3 * 12 and gb["launches"] == 12, (ga, gb)     # frames 4..15: three recordings per async frame, one per in-order frame
     assert ga["instantiations"] <= 4 and gb["instantiations"] <= 2, (ga, gb)
-    a, b = _cache_summary(wa), _cache_summary(wb)
-    m = {"alloc": (a["alloc"], b["alloc"]), "r0": (float(a["r0"].mean()), float(b["r0"].mean()))}
-    for name in ("rtdgi.spatial_filtered", "taa.this_frame_out"):
-        ia, ib = wa.image(name).astype(np.float64)[..., :3], wb.image(name).astype(np.float64)[..., :3]
-        assert np.isfinite(ia).all() and np.isfinite(ib).all(), name
-        m[name] = (float(ia.mean()), float(ib.mean()), float(np.sqrt(((ia - ib) ** 2).mean())))
-    print("async vs in-order cache chain:", m)
-    assert abs(m["alloc"][0] - m["alloc"][1]) <= 0.04 * m["alloc"][1] + 2, m
-    assert abs(m["r0"][0] - m["r0"][1]) <= 0.15 * abs(m["r0"][1]), m
-    for name in ("rtdgi.spatial_filtered", "taa.this_frame_out"):
-        ma, mb, rms = m[name]
-        assert abs(ma - mb) <= 0.08 * mb and rms <= 0.20 * mb, m
-    assert not parity.compare_images(wa, wb, names=["depth", "gbuffer", "reprojection_map", "half_depth", "half_view_normal"])
+    assert {"ircache.aux_buf", "ircache.life_buf", "ircache.grid_meta_buf2", "taa.this_frame_out"} <= set(wa.image_names())
+    assert int(wa.image("ircache.meta_buf").ravel()[3]) > 100
 
 
 def test_cuda_graph_frames_match_directly_launched_frames(cuda_lib):
