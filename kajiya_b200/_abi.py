@@ -136,6 +136,11 @@ class KjbLib:
             raise KjbError(f"{path} does not export: {self.missing}")
         if d.kjb_abi_version() != 1:
             raise KjbError("ABI version mismatch")
+        # include/kjb_tlas.h: the CUDA library and its emulator build inspect their acceleration structure; the oracle keeps its own
+        self.has_tlas_download = hasattr(d, "kjb_tlas_download")
+        if self.has_tlas_download:
+            d.kjb_tlas_download.restype = C.c_int
+            d.kjb_tlas_download.argtypes = [P, C.POINTER(C.c_uint32 * 3), C.POINTER(C.c_int32), P, P, P, P]
 
     @property
     def backend(self):

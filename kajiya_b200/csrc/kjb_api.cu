@@ -1,6 +1,9 @@
 // C-ABI entry points: context, memory, scene upload, "rebuild tlas", frame constants (include/kjb.h).
 #include "kjb_context.h"
 #include "kjb_ircache.cuh"
+#include "kjb_bvh_build.cuh"   // the device build's kernels, compiled in this translation unit
+#include "../../include/kjb_tlas.h"
+#include <algorithm>
 
 using namespace kjb;
 
@@ -68,7 +71,7 @@ int tile_mode(std::initializer_list<const TileSource*> sources) {
 // ---- "rebuild tlas" on the device.  The reference rebuilds its TLAS every frame (world_renderer.rs:865-911, ray_tracing.rs:455-520); here the
 // acceleration structure is ONE flattened world-space BVH, so a transform change means new world-space triangles and new boxes.  When only
 // transforms changed (same instances, same meshes) the topology is kept and two kernels redo the rest: (1) every leaf-order triangle record
-// is re-derived from the unified vertex buffer and its instance's 3x4 matrix — the same float operations as the host flatten, so the records
+// is re-derived from the unified vertex buffer and its instance's 3x4 matrix — the kernel that also fills the records of a full rebuild, so they
 // are bit-identical to a full rebuild's; (2) boxes are refitted bottom-up (one thread per inner node fills its leaf slots, the second arriver
 // at a node carries the union to the parent).  Hits do not depend on the topology (DESIGN.md "ray/triangle contract"), so a refitted
 // structure returns exactly what a rebuilt one would.
@@ -97,19 +100,10 @@ KJB_KERNEL(256) k_refit_tris(SceneView sc, BvhTri* tris, float* tri_box, uint32_
     tris[s] = t;
     box_of_tri(wv[0], wv[1], wv[2], tri_box + size_t(s) * 6);
 }
-KJB_DEV void write_padded_slot(BvhNode& nd, int k, const float* b) {   // Builder::padded (kjb_bvh.cpp): the slab test only culls, pad against its rounding
-    float lo[3], hi[3];
-    for (int a = 0; a < 3; ++a) {
-        const float pad = (b[3 + a] - b[a]) * 1e-5f + 1e-6f + 1e-6f * kjb_max(kjb_abs(b[a]), kjb_abs(b[3 + a]));
-        lo[a] = b[a] - pad; hi[a] = b[3 + a] + pad;
-    }
-    float* nxy = k == 0 ? nd.n0 : nd.n1;
-    nxy[0] = lo[0]; nxy[1] = hi[0]; nxy[2] = lo[1]; nxy[3] = hi[1];
-    nd.n2[k * 2 + 0] = lo[2]; nd.n2[k * 2 + 1] = hi[2];
-}
-KJB_KERNEL(256) k_refit_nodes(BvhNode* nodes, const int32_t* parent, uint32_t* count, float* slot_box, const float* tri_box, uint32_t node_count, Rows kjb_rows) {
+// node_count: the built tree's inner-node count in device memory (the grid covers the capacity)
+KJB_KERNEL(256) k_refit_nodes(BvhNode* nodes, const int32_t* parent, uint32_t* count, float* slot_box, const float* tri_box, const uint32_t* node_count, Rows kjb_rows) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= node_count) return;
+    if (i >= *node_count) return;
     uint32_t leaves = 0;
     for (int k = 0; k < 2; ++k) {
         const int32_t ch = nodes[i].child[k];
@@ -179,7 +173,7 @@ void kjb_destroy(kjb_context* c) {
     if (!c) return;
     dev_sync(c);
     dev_free(c->d_vertices); dev_free(c->d_meshes); dev_free(c->d_instances); dev_free(c->d_nodes); dev_free(c->d_tris); dev_free(c->d_tri_info);
-    dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box); dev_free(c->d_tri_box);
+    dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box); dev_free(c->d_tri_box); dev_free(c->d_bvh_scratch); dev_free(c->d_inst_prefix);
     dev_free(c->d_tex_data); dev_free(c->d_tex_desc); dev_free(c->d_lights); dev_free(c->d_ray_counters); dev_free(c->d_prev_instances); dev_free(c->d_resolve_offsets);
     for (auto& kv : c->ircache_scratch) { const auto& s = kv.second; dev_free(s.claim_rank); dev_free(s.claim_vertex); dev_free(s.life_pending); dev_free(s.scan); dev_free(s.claim_bits); dev_free(s.aux_prev); dev_free(s.entry_vertex); }
 #if !defined(KJB_EMU)
@@ -321,78 +315,121 @@ int kjb_scene_set_textures(kjb_context* c, const kjb_texture_desc* t, uint32_t n
     return dev_sync(c);
 }
 
-// "rebuild tlas": flatten every instance's triangles to world space and rebuild the BVH.  Skipped when the instance
-// list is bit-identical to the previous call (static scenes), which is the steady state of every benchmark config.
+// one slot of the pinned staging ring (4 slots): the caller's host array may change as soon as the upload is enqueued
+static void* staging_slot(kjb_context* c, size_t bytes) {
+    if (c->pinned_bytes < bytes) {
+#if !defined(KJB_EMU)
+        dev_sync(c); if (c->pinned_staging) cudaFreeHost(c->pinned_staging);
+        if (cudaMallocHost(&c->pinned_staging, bytes * 4) != cudaSuccess) { c->pinned_staging = nullptr; c->pinned_bytes = 0; return nullptr; }
+#else
+        free(c->pinned_staging); c->pinned_staging = malloc(bytes * 4);
+#endif
+        c->pinned_bytes = bytes;
+    }
+    return (char*)c->pinned_staging + size_t(c->staging_seq++ & 3u) * c->pinned_bytes;
+}
+// grow-only device capacities of the structure and its build: past the first frames of a scene, a rebuild allocates nothing
+static int reserve_tlas(kjb_context* c, uint32_t tris, uint32_t instances) {
+    const bool grow_tris = tris > c->bvh_tri_cap || !c->d_bvh_scratch, grow_inst = instances + 1 > c->bvh_inst_cap || !c->d_instances;
+    if (!grow_tris && !grow_inst) return 0;
+    dev_sync(c);
+    if (grow_inst) {
+        const uint32_t cap = std::max(instances + 1, c->bvh_inst_cap * 2);
+        dev_free(c->d_instances); dev_free(c->d_inst_prefix);
+        c->d_instances = (kjb_instance*)dev_alloc(size_t(cap) * sizeof(kjb_instance)); c->d_inst_prefix = (uint32_t*)dev_alloc(size_t(cap + 1) * 4);
+        c->bvh_inst_cap = cap;
+        if (!c->d_instances || !c->d_inst_prefix) { c->bvh_inst_cap = 0; return c->fail("kjb_rebuild_tlas: out of device memory"); }
+    }
+    if (grow_tris) {
+        const uint32_t cap = std::max(std::max(tris, 1u), c->bvh_tri_cap + c->bvh_tri_cap / 2);
+        dev_free(c->d_nodes); dev_free(c->d_tris); dev_free(c->d_tri_info); dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box);
+        dev_free(c->d_tri_box); dev_free(c->d_bvh_scratch);
+        c->d_nodes = (BvhNode*)dev_alloc(size_t(cap) * sizeof(BvhNode)); c->d_tris = (BvhTri*)dev_alloc(size_t(cap) * sizeof(BvhTri));
+        c->d_tri_info = (TriInfo*)dev_alloc(size_t(cap + 1) * sizeof(TriInfo)); c->d_node_parent = (int32_t*)dev_alloc(size_t(cap) * 4);
+        c->d_refit_count = (uint32_t*)dev_alloc(size_t(cap) * 4); c->d_slot_box = (float*)dev_alloc(size_t(cap) * 12 * sizeof(float));
+        c->d_tri_box = (float*)dev_alloc(size_t(cap) * 6 * sizeof(float)); c->d_bvh_scratch = dev_alloc(bvh_build_scratch_bytes(cap));
+        c->bvh_tri_cap = cap;
+        if (!c->d_nodes || !c->d_tris || !c->d_tri_info || !c->d_node_parent || !c->d_refit_count || !c->d_slot_box || !c->d_tri_box || !c->d_bvh_scratch) {
+            c->bvh_tri_cap = 0; return c->fail("kjb_rebuild_tlas: out of device memory");
+        }
+        c->d_node_count = bvh_build_node_count(c);
+    }
+    return 0;
+}
+
+// "rebuild tlas": the instances' triangles in world space and the BVH over them, built on the device (kjb_bvh_build.cuh).  Skipped when the
+// instance list is bit-identical to the previous call (static scenes), which is the steady state of every benchmark config.
 int kjb_rebuild_tlas(kjb_context* c, const kjb_instance* inst, uint32_t n) {
     if (c->tlas_valid && c->h_instances.size() == n && (n == 0 || memcmp(c->h_instances.data(), inst, n * sizeof(kjb_instance)) == 0)) return 0;
     {   // same instances, same meshes, other transforms (the per-frame case of a moving scene): refit on the device, no host work, no sync
         bool same_topology = c->tlas_valid && c->h_instances.size() == n && n > 0 && c->node_count > 0 && c->d_node_parent;
         for (uint32_t i = 0; same_topology && i < n; ++i) same_topology = c->h_instances[i].mesh_index == inst[i].mesh_index;
         if (same_topology) {
-            // the instance array the kernels read is double-buffered through a pinned staging copy so that the caller's array may change at once
-            if (c->pinned_bytes < n * sizeof(kjb_instance)) {
-#if !defined(KJB_EMU)
-                dev_sync(c); if (c->pinned_staging) cudaFreeHost(c->pinned_staging);
-                if (cudaMallocHost(&c->pinned_staging, n * sizeof(kjb_instance) * 4) != cudaSuccess) { c->pinned_staging = nullptr; c->pinned_bytes = 0; return c->fail("kjb_rebuild_tlas: pinned staging allocation failed"); }
-#else
-                free(c->pinned_staging); c->pinned_staging = malloc(n * sizeof(kjb_instance) * 4);
-#endif
-                c->pinned_bytes = n * sizeof(kjb_instance);
-            }
-            kjb_instance* stage = (kjb_instance*)c->pinned_staging + size_t(c->tlas_refits & 3u) * n;
+            kjb_instance* stage = (kjb_instance*)staging_slot(c, n * sizeof(kjb_instance));
+            if (!stage) return c->fail("kjb_rebuild_tlas: pinned staging allocation failed");
             memcpy(stage, inst, n * sizeof(kjb_instance));
             c->h_instances.assign(inst, inst + n);
             if (dev_h2d(c, c->d_instances, stage, n * sizeof(kjb_instance))) return c->fail("kjb_rebuild_tlas: instance upload failed");
             dev_memset(c, c->d_refit_count, 0, c->node_count * sizeof(uint32_t));
             const kjb::Rows kjb__rows = {0, 1};
             KJB_LAUNCH(c, k_refit_tris, KJB_DIMS(dim3((c->slot_count + 255) / 256), dim3(256)), c->g.scene, c->d_tris, c->d_tri_box, c->slot_count);
-            KJB_LAUNCH(c, k_refit_nodes, KJB_DIMS(dim3((c->node_count + 255) / 256), dim3(256)), c->d_nodes, (const int32_t*)c->d_node_parent, c->d_refit_count, c->d_slot_box, (const float*)c->d_tri_box, c->node_count);
+            KJB_LAUNCH(c, k_refit_nodes, KJB_DIMS(dim3((c->node_count + 255) / 256), dim3(256)), c->d_nodes, (const int32_t*)c->d_node_parent, c->d_refit_count, c->d_slot_box, (const float*)c->d_tri_box, (const uint32_t*)c->d_node_count);
             c->tlas_refits++;
             KJB_PASS_EPILOGUE(c, "rebuild tlas (refit)");
         }
     }
-    dev_sync(c);
-    c->tlas_rebuilds++;
-    c->h_instances.assign(inst, inst + n);
-    std::vector<float> wt; std::vector<TriInfo> info;
-    { size_t total = 0; for (uint32_t i = 0; i < n; ++i) if (inst[i].mesh_index < c->h_meshes.size()) total += c->h_index_counts[inst[i].mesh_index] / 3; wt.reserve(total * 9); info.reserve(total); }
+    // a new instance list: the triangle count and each instance's first triangle are known here, everything else is built on the device
+    uint64_t total = 0;
     for (uint32_t i = 0; i < n; ++i) {
         if (inst[i].mesh_index >= c->h_meshes.size()) return c->fail("kjb_rebuild_tlas: instance references an unknown mesh");
-        const kjb_gpu_mesh& m = c->h_meshes[inst[i].mesh_index];
-        const uint32_t ntri = c->h_index_counts[inst[i].mesh_index] / 3;
-        const uint8_t* vb = c->h_vertices.data();
-        for (uint32_t p = 0; p < ntri; ++p) {
-            for (int k = 0; k < 3; ++k) {
-                uint32_t idx; memcpy(&idx, vb + m.index_offset + (p * 3 + k) * 4, 4);
-                float v[3]; memcpy(v, vb + m.vertex_core_offset + size_t(idx) * 16, 12);
-                const float3 w = xform_point(inst[i].transform, f3(v[0], v[1], v[2]));
-                wt.push_back(w.x); wt.push_back(w.y); wt.push_back(w.z);
-            }
-            TriInfo ti; ti.instance = i; ti.prim = p; info.push_back(ti);
-        }
+        total += c->h_index_counts[inst[i].mesh_index] / 3;
     }
-    HostBvh bvh;
-    build_bvh(wt.data(), info.data(), uint32_t(info.size()), bvh);
-    dev_free(c->d_nodes); dev_free(c->d_tris); dev_free(c->d_tri_info); dev_free(c->d_instances);
-    dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box); dev_free(c->d_tri_box);
-    c->node_count = uint32_t(bvh.nodes.size()); c->slot_count = uint32_t(bvh.tris.size());
-    c->d_node_parent = c->node_count ? (int32_t*)dev_alloc(c->node_count * sizeof(int32_t)) : nullptr;
-    c->d_refit_count = c->node_count ? (uint32_t*)dev_alloc(c->node_count * sizeof(uint32_t)) : nullptr;
-    c->d_slot_box = c->node_count ? (float*)dev_alloc(size_t(c->node_count) * 12 * sizeof(float)) : nullptr;
-    c->d_tri_box = (float*)dev_alloc(size_t(c->slot_count) * 6 * sizeof(float));
-    if (c->d_node_parent) dev_h2d(c, c->d_node_parent, bvh.parent.data(), c->node_count * sizeof(int32_t));
-    c->d_nodes = bvh.nodes.empty() ? nullptr : (BvhNode*)dev_alloc(bvh.nodes.size() * sizeof(BvhNode));
-    c->d_tris = (BvhTri*)dev_alloc(bvh.tris.size() * sizeof(BvhTri));
-    c->d_tri_info = (TriInfo*)dev_alloc((bvh.info.size() + 1) * sizeof(TriInfo));
-    c->d_instances = (kjb_instance*)dev_alloc((n + 1) * sizeof(kjb_instance));
-    if (c->d_nodes) dev_h2d(c, c->d_nodes, bvh.nodes.data(), bvh.nodes.size() * sizeof(BvhNode));
-    dev_h2d(c, c->d_tris, bvh.tris.data(), bvh.tris.size() * sizeof(BvhTri));
-    if (!bvh.info.empty()) dev_h2d(c, c->d_tri_info, bvh.info.data(), bvh.info.size() * sizeof(TriInfo));
-    if (n) dev_h2d(c, c->d_instances, inst, n * sizeof(kjb_instance));
+    if (total >= (1u << 28)) return c->fail("kjb_rebuild_tlas: more than 2^28 triangles (leaf references hold 28 bits of triangle slot)");
+    const uint32_t ntri = uint32_t(total);
+    if (reserve_tlas(c, ntri, n)) return 1;
+    const size_t inst_bytes = size_t(n) * sizeof(kjb_instance), stage_bytes = inst_bytes + size_t(n + 1) * 4;
+    uint8_t* stage = (uint8_t*)staging_slot(c, stage_bytes);
+    if (!stage) return c->fail("kjb_rebuild_tlas: pinned staging allocation failed");
+    memcpy(stage, inst, inst_bytes);
+    uint32_t* prefix = (uint32_t*)(stage + inst_bytes);
+    prefix[0] = 0;
+    for (uint32_t i = 0; i < n; ++i) prefix[i + 1] = prefix[i] + c->h_index_counts[inst[i].mesh_index] / 3;
+    if ((n && dev_h2d(c, c->d_instances, stage, inst_bytes)) || dev_h2d(c, c->d_inst_prefix, prefix, size_t(n + 1) * 4)) return c->fail("kjb_rebuild_tlas: instance upload failed");
+    c->tlas_rebuilds++;
+    c->h_instances.assign(inst, inst + n);
     c->g.scene.nodes = c->d_nodes; c->g.scene.tris = c->d_tris; c->g.scene.tri_info = c->d_tri_info; c->g.scene.instances = c->d_instances;
-    c->g.scene.tri_count = uint32_t(info.size()); c->g.scene.root = bvh.root_child;
+    c->g.scene.tri_count = ntri;
+    // the root is known from the count alone: none (one all-zero triangle record that never hits), a single leaf, or inner node 0
+    c->g.scene.root = ntri == 0 ? ~int32_t(0) : (ntri <= 4 ? ~int32_t(ntri - 1) : 0);
+    c->slot_count = ntri ? ntri : 1;
+    c->node_count = ntri > 4 ? ntri - 1 : 0;   // a bound: the refit reads the built count from d_node_count
     c->tlas_valid = true;
-    return dev_sync(c);
+    if (ntri == 0) {
+        if (dev_memset(c, c->d_tris, 0, sizeof(BvhTri))) return c->fail("kjb_rebuild_tlas: memset failed");
+        KJB_PASS_EPILOGUE(c, "rebuild tlas");
+    }
+    if (bvh_build_on_device(c, n, ntri)) return 1;
+    const kjb::Rows kjb__rows = {0, 1};
+    KJB_LAUNCH(c, k_refit_tris, KJB_DIMS(dim3((ntri + 255) / 256), dim3(256)), c->g.scene, c->d_tris, c->d_tri_box, ntri);
+    KJB_PASS_EPILOGUE(c, "rebuild tlas");
+}
+
+// Copies the structure to the host for inspection (synchronous; not for the frame loop).  Null arrays are skipped; the counts are always written.
+int kjb_tlas_download(kjb_context* c, uint32_t out_counts[3], int32_t* out_root, void* nodes, void* tris, void* tri_info, int32_t* parent) {
+    if (dev_sync(c)) return c->fail("kjb_tlas_download: sync failed");
+    uint32_t nodes_n = 0;
+    if (c->tlas_valid && c->node_count) dev_d2h(c, &nodes_n, c->d_node_count, 4);
+    if (dev_sync(c)) return c->fail("kjb_tlas_download: sync failed");
+    const uint32_t slots = c->tlas_valid ? c->slot_count : 0, infos = c->tlas_valid ? c->g.scene.tri_count : 0;
+    out_counts[0] = nodes_n; out_counts[1] = slots; out_counts[2] = infos;
+    if (out_root) *out_root = c->g.scene.root;
+    if (nodes && nodes_n) dev_d2h(c, nodes, c->d_nodes, size_t(nodes_n) * sizeof(BvhNode));
+    if (parent && nodes_n) dev_d2h(c, parent, c->d_node_parent, size_t(nodes_n) * 4);
+    if (tris && slots) dev_d2h(c, tris, c->d_tris, size_t(slots) * sizeof(BvhTri));
+    if (tri_info && infos) dev_d2h(c, tri_info, c->d_tri_info, size_t(infos) * sizeof(TriInfo));
+    if (dev_sync(c)) return c->fail("kjb_tlas_download: sync failed");
+    const char* e = dev_check(c); if (e) return c->fail(std::string("kjb_tlas_download: ") + e);
+    return 0;
 }
 
 #if defined(KJB_EMU)

@@ -1,11 +1,22 @@
-// Host-side binned-SAH BVH2 builder (see kjb_bvh.h).  Scene preparation, not the hot path: runs when geometry or
-// instance transforms change ("rebuild tlas"), never per ray.
+// Host binned-SAH BVH2 builder: the reference the device build (kjb_bvh_build.cuh) is checked against — same nodes and parent links byte
+// for byte, same tri_info, same triangles per leaf.  The library ran this builder before the structure was built on the device; the CUDA
+// library no longer compiles it.  Only the test emulator's build links it, which exports it as kjb_ref_* (bottom of this file).
 #include "kjb_bvh.h"
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <vector>
 
 namespace kjb {
+
+struct HostBvh {
+    std::vector<BvhNode> nodes;
+    std::vector<BvhTri> tris;        // leaf order
+    std::vector<TriInfo> info;       // by gid
+    int32_t root_child = 0;          // encoded like a child reference (a 1-leaf scene has no inner node)
+    std::vector<int32_t> parent;     // per inner node: (parent node << 1) | child slot, -1 for the root
+};
+
 namespace {
 
 struct Box {
@@ -124,3 +135,25 @@ void build_bvh(const float* world_tris, const TriInfo* info, uint32_t tri_count,
 }
 
 }  // namespace kjb
+
+// ---- C exports for the tests (emulator build only): build from gid-ordered world-space triangles (float[9] each), read the result back
+extern "C" {
+void* kjb_ref_bvh_build(const float* world_tris, uint32_t tri_count) {
+    std::vector<kjb::TriInfo> info(tri_count);
+    for (uint32_t t = 0; t < tri_count; ++t) { info[t].instance = 0; info[t].prim = t; }
+    kjb::HostBvh* h = new kjb::HostBvh();
+    kjb::build_bvh(world_tris, info.data(), tri_count, *h);
+    return h;
+}
+void kjb_ref_bvh_counts(void* p, uint32_t out[2], int32_t* root) {
+    const kjb::HostBvh* h = (const kjb::HostBvh*)p;
+    out[0] = uint32_t(h->nodes.size()); out[1] = uint32_t(h->tris.size()); *root = h->root_child;
+}
+void kjb_ref_bvh_copy(void* p, void* nodes, void* tris, int32_t* parent) {
+    const kjb::HostBvh* h = (const kjb::HostBvh*)p;
+    memcpy(nodes, h->nodes.data(), h->nodes.size() * sizeof(kjb::BvhNode));
+    memcpy(tris, h->tris.data(), h->tris.size() * sizeof(kjb::BvhTri));
+    memcpy(parent, h->parent.data(), h->parent.size() * sizeof(int32_t));
+}
+void kjb_ref_bvh_free(void* p) { delete (kjb::HostBvh*)p; }
+}

@@ -8,25 +8,14 @@
 //   n0 = (c0.lo.x, c0.hi.x, c0.lo.y, c0.hi.y)   n1 = (c1.lo.x, c1.hi.x, c1.lo.y, c1.hi.y)
 //   n2 = (c0.lo.z, c0.hi.z, c1.lo.z, c1.hi.z)   n3 = (child0, child1, -, -) as int bits; child < 0 => leaf ~((first << 3) | (count - 1))
 // Triangles are stored in leaf order as 48-byte records (v0 | global id, e1, e2) in world space.
+// Built on the device (kjb_bvh_build.cuh), refitted on the device when only transforms change (kjb_api.cu).
 #pragma once
 #include <stdint.h>
-#include <vector>
 
 namespace kjb {
 
 struct BvhNode { float n0[4], n1[4], n2[4]; int32_t child[4]; };          // 64 B
 struct BvhTri { float v0[3]; uint32_t gid; float e1[3]; uint32_t pad0; float e2[3]; uint32_t pad1; };   // 48 B
 struct TriInfo { uint32_t instance, prim; };                               // indexed by global triangle id
-
-struct HostBvh {
-    std::vector<BvhNode> nodes;
-    std::vector<BvhTri> tris;        // leaf order
-    std::vector<TriInfo> info;       // by gid
-    int32_t root_child = 0;          // encoded like a child reference (a 1-leaf scene has no inner node)
-    std::vector<int32_t> parent;     // per inner node: (parent node << 1) | child slot, -1 for the root — what the device refit walks upwards
-};
-
-// world_tris: gid-ordered (instance-major) triangles as (v0, v1, v2) float[9].  Binned-SAH build, leaves of <= 4 triangles.
-void build_bvh(const float* world_tris, const TriInfo* info, uint32_t tri_count, HostBvh& out);
 
 }  // namespace kjb

@@ -36,6 +36,10 @@ struct kjb_context {
     // device refit of the acceleration structure when only instance transforms change ("rebuild tlas" every frame, kjb_api.cu)
     int32_t* d_node_parent = nullptr; uint32_t* d_refit_count = nullptr; float* d_slot_box = nullptr; float* d_tri_box = nullptr; uint32_t node_count = 0, slot_count = 0;
     uint64_t tlas_refits = 0, tlas_rebuilds = 0;
+    // device build of the structure (kjb_bvh_build.cuh): grow-only capacities in triangles and instances, so that a rebuild with enough
+    // room neither allocates nor synchronises; node_count above is then the capacity bound and d_node_count the built tree's count
+    uint32_t bvh_tri_cap = 0, bvh_inst_cap = 0; void* d_bvh_scratch = nullptr; uint32_t* d_inst_prefix = nullptr; uint32_t* d_node_count = nullptr;
+    uint64_t staging_seq = 0;   // slot of the pinned staging ring the next instance upload uses
     uint8_t* d_tex_data = nullptr; uint4* d_tex_desc = nullptr; uint32_t tex_count = 0;
     kjb_triangle_light* d_lights = nullptr; uint32_t lights_capacity = 0;
     unsigned long long* d_ray_counters = nullptr;

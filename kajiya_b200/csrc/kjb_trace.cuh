@@ -14,6 +14,19 @@ namespace kjb {
 struct Ray { float3 origin, dir; float tmin, tmax; };
 struct HitInfo { bool hit; float t, u, v; uint32_t gid; };
 
+// child slot k of a node from the exact box b = (lo, hi): the slab test only culls, so the box is padded against its rounding.  The device
+// build (kjb_bvh_build.cuh) and the refit (kjb_api.cu) both write every box through here.
+KJB_DEV void write_padded_slot(BvhNode& nd, int k, const float* b) {
+    float lo[3], hi[3];
+    for (int a = 0; a < 3; ++a) {
+        const float pad = (b[3 + a] - b[a]) * 1e-5f + 1e-6f + 1e-6f * kjb_max(kjb_abs(b[a]), kjb_abs(b[3 + a]));
+        lo[a] = b[a] - pad; hi[a] = b[3 + a] + pad;
+    }
+    float* nxy = k == 0 ? nd.n0 : nd.n1;
+    nxy[0] = lo[0]; nxy[1] = hi[0]; nxy[2] = lo[1]; nxy[3] = hi[1];
+    nd.n2[k * 2 + 0] = lo[2]; nd.n2[k * 2 + 1] = hi[2];
+}
+
 KJB_DEV float4 ldg4(const float* p) {
 #if defined(__CUDA_ARCH__)
     return __ldg(reinterpret_cast<const float4*>(p));

@@ -222,6 +222,19 @@ class World:
         self._check(self.d.kjb_tlas_stats(self.ctx, C.byref(s)))
         return dict(rebuilds=s[0], refits=s[1])
 
+    def tlas_download(self):
+        """the acceleration structure as built (include/kjb_tlas.h): dict of raw arrays — nodes uint32[n, 16] (64-byte nodes), tris
+        uint32[slots, 12] (48-byte leaf-order records, global id in word 3), tri_info uint32[triangles, 2] (instance, primitive), parent
+        int32[n] — and root (a node index, or a leaf / empty reference)"""
+        if not self.lib.has_tlas_download:
+            raise KjbError(f"{self.lib.backend} does not expose its acceleration structure")
+        counts, root = (C.c_uint32 * 3)(), C.c_int32()
+        self._check(self.d.kjb_tlas_download(self.ctx, C.byref(counts), C.byref(root), None, None, None, None))
+        nodes, tris = np.zeros((counts[0], 16), np.uint32), np.zeros((counts[1], 12), np.uint32)
+        info, parent = np.zeros((counts[2], 2), np.uint32), np.zeros(counts[0], np.int32)
+        self._check(self.d.kjb_tlas_download(self.ctx, C.byref(counts), C.byref(root), nodes.ctypes.data, tris.ctypes.data, info.ctypes.data, parent.ctypes.data))
+        return dict(nodes=nodes, tris=tris, tri_info=info, parent=parent, root=int(root.value))
+
     # -- images ------------------------------------------------------------------------------------------------
     def image_names(self):
         return [n for n in self.d.kjb_world_image_names(self.w).decode().split("\n") if n]
