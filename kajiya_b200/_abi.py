@@ -141,6 +141,10 @@ class KjbLib:
         if self.has_tlas_download:
             d.kjb_tlas_download.restype = C.c_int
             d.kjb_tlas_download.argtypes = [P, C.POINTER(C.c_uint32 * 3), C.POINTER(C.c_int32), P, P, P, P]
+        self.has_tlas_trace = hasattr(d, "kjb_tlas_trace")
+        if self.has_tlas_trace:
+            d.kjb_tlas_trace.restype = C.c_int
+            d.kjb_tlas_trace.argtypes = [P, P, C.c_uint32, C.c_uint32, P]
 
     @property
     def backend(self):

@@ -432,6 +432,51 @@ int kjb_tlas_download(kjb_context* c, uint32_t out_counts[3], int32_t* out_root,
     return 0;
 }
 
+}  // extern "C"
+// one thread per ray: the frame's walk (trace), or intersect_leaf over every triangle record, whose selection rule does not depend on the order
+KJB_KERNEL(128) k_tlas_trace(SceneView sc, const float* rays, uint32_t n, uint32_t flags, uint32_t slots, uint32_t* out, Rows kjb_rows) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float* p = rays + size_t(i) * 8;
+    Ray r; r.origin = f3(p[0], p[1], p[2]); r.tmin = p[3]; r.dir = f3(p[4], p[5], p[6]); r.tmax = p[7];
+    const bool any = flags & KJB_TLAS_TRACE_ANY_HIT, cull = flags & KJB_TLAS_TRACE_CULL_BACK;
+    HitInfo h; h.hit = false; h.t = r.tmax; h.u = 0; h.v = 0; h.gid = 0xffffffffu;
+    if (flags & KJB_TLAS_TRACE_BRUTE_FORCE) {
+        if (any) h.hit = intersect_leaf<true>(sc.tris, 0, slots, r, cull, h);
+        else intersect_leaf<false>(sc.tris, 0, slots, r, cull, h);
+    } else {
+        h = any ? trace<true>(sc, r, cull) : trace<false>(sc, r, cull);
+    }
+    uint32_t* o = out + size_t(i) * 4;
+    if (!h.hit) { o[0] = 0; o[1] = 0; o[2] = 0; o[3] = 0xffffffffu; }
+    else if (any) { o[0] = 0; o[1] = 0; o[2] = 0; o[3] = 0; }
+    else { o[0] = kjb_f2u(h.t); o[1] = kjb_f2u(h.u); o[2] = kjb_f2u(h.v); o[3] = h.gid; }
+}
+extern "C" {
+
+// Inspection call for tests (synchronous, allocates per call).
+int kjb_tlas_trace(kjb_context* c, const float* rays, uint32_t n, uint32_t flags, float* out) {
+    if (!c->tlas_valid) return c->fail("kjb_tlas_trace: no acceleration structure (render a frame or call kjb_rebuild_tlas first)");
+    if (flags & ~(KJB_TLAS_TRACE_ANY_HIT | KJB_TLAS_TRACE_CULL_BACK | KJB_TLAS_TRACE_BRUTE_FORCE)) return c->fail("kjb_tlas_trace: unknown flags");
+    if (n == 0) return 0;
+    if (dev_sync(c)) return c->fail("kjb_tlas_trace: sync failed");
+    float* d_rays = (float*)dev_alloc(size_t(n) * 8 * sizeof(float));
+    uint32_t* d_out = (uint32_t*)dev_alloc(size_t(n) * 4 * sizeof(uint32_t));
+    int rc = 0;
+    if (!d_rays || !d_out) rc = c->fail("kjb_tlas_trace: out of device memory");
+    if (!rc && dev_h2d(c, d_rays, rays, size_t(n) * 8 * sizeof(float))) rc = c->fail("kjb_tlas_trace: upload failed");
+    if (!rc) {
+        const kjb::Rows kjb__rows = {0, 1};
+        KJB_LAUNCH(c, k_tlas_trace, KJB_DIMS(dim3((n + 127) / 128), dim3(128)), c->g.scene, (const float*)d_rays, n, flags, c->slot_count, d_out);
+        if (dev_d2h(c, out, d_out, size_t(n) * 4 * sizeof(uint32_t))) rc = c->fail("kjb_tlas_trace: download failed");
+    }
+    if (dev_sync(c) && !rc) rc = c->fail("kjb_tlas_trace: sync failed");
+    const char* e = dev_check(c);
+    if (e && !rc) rc = c->fail(std::string("kjb_tlas_trace: ") + e);
+    dev_free(d_rays); dev_free(d_out);
+    return rc;
+}
+
 #if defined(KJB_EMU)
 int kjb_graph_begin(kjb_context*) { return 0; }
 int kjb_graph_end(kjb_context*) { return 0; }

@@ -65,6 +65,24 @@ KJB_DEV bool intersect_leaf(const BvhTri* tris, uint32_t first, uint32_t count, 
 // the slab test's min/max are kjb_min / kjb_max: one FMNMX each on the device (include/kjb_numeric.h)
 #define KJB_SLAB_MIN kjb_min
 #define KJB_SLAB_MAX kjb_max
+
+// Culling slack: a child is kept when tn*(1 - s) <= min(tf, best.t)*(1 + s) (signs handled), s = KJB_SLAB_SLACK_K * 2^-24 = u * k.  Padding
+// alone cannot keep culling conservative: the slab terms round relative to |plane - origin| (far origins), and the Moeller-Trumbore t of a
+// triangle lying on its box's face (floors, walls: flat boxes) can come out below the computed box entry.  The bound, to first order in u:
+//  * slab: c = (plane - o) * (1/d) is three roundings, min/max are exact, so the computed tn <= tn + 3u|tn| and tf >= tf - 3u|tf|;
+//    the slack multiply is one more rounding;
+//  * Moeller-Trumbore (kjb_device.cuh: cross without fma, dot with two fma): N = dot(e2, cross(o - v0, e1)) carries 6 roundings,
+//    det = dot(e1, cross(d, e2)) 5, each at most 1.155 (= 2/sqrt 3, the largest |a||b||c|-normalised absolute triple product) of
+//    u|a||b||c|; then 1/det and N*inv.  With S = |e1||e2| / |e1 x e2| (triangle shape), cos = the cosine between d and the normal and
+//    rho = |o - v0| / (t|d|), the relative error of t is  delta <= (1.155 (6 rho + 5) S / |cos| + 2) u.
+// A triangle whose exact hit lies in the box is therefore never culled while delta + 4u <= s, i.e. 1.155 (6 rho + 5) S / |cos| <= k - 6:
+// with k = 2^14, S / |cos| <= 1290 for rho = 1 (origin far from the triangle) and <= 1010 for rho = 1.5.  Rays beyond that (grazing,
+// slivers, origins close to a large triangle) may still lose a near-tie to topology; tests/test_ray_contract.py tags them ill-conditioned.
+// Each bound is one FFMA with an |t| operand, rounded once: t - s|t|, t + s|t|.  An infinite tn = +inf or tf = -inf turns into NaN, which
+// fails tn <= tf as the infinity would have.
+#define KJB_SLAB_SLACK_K 16384.0f
+KJB_DEV float slab_near(float t) { return kjb_fma(-KJB_SLAB_SLACK_K * 0x1p-24f, kjb_abs(t), t); }
+KJB_DEV float slab_far(float t) { return kjb_fma(KJB_SLAB_SLACK_K * 0x1p-24f, kjb_abs(t), t); }
 template <bool ANY_HIT>
 KJB_DEV HitInfo trace(const SceneView& sc, const Ray& r, bool cull_back) {
     HitInfo best; best.hit = false; best.t = r.tmax; best.u = 0; best.v = 0; best.gid = 0xffffffffu;
@@ -94,10 +112,10 @@ KJB_DEV HitInfo trace(const SceneView& sc, const Ray& r, bool cull_back) {
             const float c1loy = (n1.z - r.origin.y) * inv_dir.y, c1hiy = (n1.w - r.origin.y) * inv_dir.y;
             const float c1loz = (n2.z - r.origin.z) * inv_dir.z, c1hiz = (n2.w - r.origin.z) * inv_dir.z;
             const float tmax_cur = ANY_HIT ? r.tmax : best.t;
-            const float t0n = KJB_SLAB_MAX(KJB_SLAB_MAX(KJB_SLAB_MIN(c0lox, c0hix), KJB_SLAB_MIN(c0loy, c0hiy)), KJB_SLAB_MAX(KJB_SLAB_MIN(c0loz, c0hiz), r.tmin));
-            const float t0f = KJB_SLAB_MIN(KJB_SLAB_MIN(KJB_SLAB_MAX(c0lox, c0hix), KJB_SLAB_MAX(c0loy, c0hiy)), KJB_SLAB_MIN(KJB_SLAB_MAX(c0loz, c0hiz), tmax_cur));
-            const float t1n = KJB_SLAB_MAX(KJB_SLAB_MAX(KJB_SLAB_MIN(c1lox, c1hix), KJB_SLAB_MIN(c1loy, c1hiy)), KJB_SLAB_MAX(KJB_SLAB_MIN(c1loz, c1hiz), r.tmin));
-            const float t1f = KJB_SLAB_MIN(KJB_SLAB_MIN(KJB_SLAB_MAX(c1lox, c1hix), KJB_SLAB_MAX(c1loy, c1hiy)), KJB_SLAB_MIN(KJB_SLAB_MAX(c1loz, c1hiz), tmax_cur));
+            const float t0n = slab_near(KJB_SLAB_MAX(KJB_SLAB_MAX(KJB_SLAB_MIN(c0lox, c0hix), KJB_SLAB_MIN(c0loy, c0hiy)), KJB_SLAB_MAX(KJB_SLAB_MIN(c0loz, c0hiz), r.tmin)));
+            const float t0f = slab_far(KJB_SLAB_MIN(KJB_SLAB_MIN(KJB_SLAB_MAX(c0lox, c0hix), KJB_SLAB_MAX(c0loy, c0hiy)), KJB_SLAB_MIN(KJB_SLAB_MAX(c0loz, c0hiz), tmax_cur)));
+            const float t1n = slab_near(KJB_SLAB_MAX(KJB_SLAB_MAX(KJB_SLAB_MIN(c1lox, c1hix), KJB_SLAB_MIN(c1loy, c1hiy)), KJB_SLAB_MAX(KJB_SLAB_MIN(c1loz, c1hiz), r.tmin)));
+            const float t1f = slab_far(KJB_SLAB_MIN(KJB_SLAB_MIN(KJB_SLAB_MAX(c1lox, c1hix), KJB_SLAB_MAX(c1loy, c1hiy)), KJB_SLAB_MIN(KJB_SLAB_MAX(c1loz, c1hiz), tmax_cur)));
             const bool h0 = t0n <= t0f, h1 = t1n <= t1f;
             if (h0 && h1) {
                 const bool near0 = t0n <= t1n;

@@ -235,6 +235,18 @@ class World:
         self._check(self.d.kjb_tlas_download(self.ctx, C.byref(counts), C.byref(root), nodes.ctypes.data, tris.ctypes.data, info.ctypes.data, parent.ctypes.data))
         return dict(nodes=nodes, tris=tris, tri_info=info, parent=parent, root=int(root.value))
 
+    def trace_rays(self, rays, any_hit=False, cull_back=False, brute_force=False):
+        """rays float32[n, 8] (o.xyz, tmin, d.xyz, tmax) against the structure as built (include/kjb_tlas.h: kjb_tlas_trace) -> uint32[n, 4]:
+        t, u, v as float bits and the global triangle id, (0, 0, 0, 0xffffffff) for a miss; with any_hit only column 3 counts (0 = hit).
+        brute_force tests every triangle record instead of walking the tree."""
+        if not self.lib.has_tlas_trace:
+            raise KjbError(f"{self.lib.backend} does not expose its acceleration structure")
+        r = np.ascontiguousarray(rays, np.float32).reshape(-1, 8)
+        out = np.zeros((len(r), 4), np.uint32)
+        flags = (1 if any_hit else 0) | (2 if cull_back else 0) | (4 if brute_force else 0)   # KJB_TLAS_TRACE_*
+        self._check(self.d.kjb_tlas_trace(self.ctx, r.ctypes.data, len(r), flags, out.ctypes.data))
+        return out
+
     # -- images ------------------------------------------------------------------------------------------------
     def image_names(self):
         return [n for n in self.d.kjb_world_image_names(self.w).decode().split("\n") if n]

@@ -137,6 +137,23 @@ int kjo_trace_closest(kjb_context* c, const float* rays /* n x 8: o.xyz, tmin, d
     }
     return 0;
 }
+// The same with u, v, any-hit and back-face culling.  Rays and results as kjb_tlas_trace (include/kjb_tlas.h): n x 8 floats
+// (o.xyz, tmin, d.xyz, tmax) in, n x 4 words (t, u, v bits, triangle id; 0, 0, 0, ~0 for a miss) out; with any_hit only word 3 counts (0 = hit).
+int kjo_trace_rays(kjb_context* c, const float* rays, uint32_t n, int brute, int any_hit, int cull_back, uint32_t* out) {
+    for (uint32_t i = 0; i < n; ++i) {
+        Ray r; r.origin = float3(rays[i * 8], rays[i * 8 + 1], rays[i * 8 + 2]); r.tmin = rays[i * 8 + 3];
+        r.dir = float3(rays[i * 8 + 4], rays[i * 8 + 5], rays[i * 8 + 6]); r.tmax = rays[i * 8 + 7];
+        uint32_t* o = out + size_t(i) * 4;
+        o[0] = o[1] = o[2] = 0; o[3] = 0xffffffffu;
+        if (any_hit) {
+            if (brute ? c->scene.closest_brute(r, cull_back != 0).hit : c->scene.any_hit(r, cull_back != 0)) o[3] = 0;
+            continue;
+        }
+        Scene::HitInfo h = brute ? c->scene.closest_brute(r, cull_back != 0) : c->scene.closest(r, cull_back != 0);
+        if (h.hit) { o[0] = asuint(h.t); o[1] = asuint(h.u); o[2] = asuint(h.v); o[3] = h.tri; }
+    }
+    return 0;
+}
 
 }  // extern "C"
 

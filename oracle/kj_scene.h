@@ -93,8 +93,9 @@ struct Scene {
             lo = min(lo, a); hi = max(hi, b);
             float3 c = (a + b) * 0.5f; clo = min(clo, c); chi = max(chi, c);
         }
-        // pad the box a little: the slab test only culls, it must never reject a true hit
-        float3 pad = (hi - lo) * 1e-5f + float3(1e-6f);
+        // pad the box a little against the slab test's rounding (the product's padding: the |b| term keeps the pad above one ulp of the
+        // box's own coordinates, so a flat box far from the origin stays a slab of non-zero width)
+        float3 pad = (hi - lo) * 1e-5f + float3(1e-6f) + max(abs(lo), abs(hi)) * 1e-6f;
         nodes[idx].bmin = lo - pad; nodes[idx].bmax = hi + pad;
         if (count <= 4) { nodes[idx].first = first; nodes[idx].count = count; nodes[idx].left = nodes[idx].right = -1; return idx; }
         float3 ext = chi - clo;
@@ -130,11 +131,16 @@ struct Scene {
     static bool ray_has_nan(const Ray& r) {
         return !(r.dir.x == r.dir.x && r.dir.y == r.dir.y && r.dir.z == r.dir.z && r.origin.x == r.origin.x && r.origin.y == r.origin.y && r.origin.z == r.origin.z && r.tmin == r.tmin && r.tmax == r.tmax);
     }
+    // The culling slack of the product's walk (kajiya_b200/csrc/kjb_trace.cuh, where its error bound is written out): the interval is
+    // widened by s = k * 2^-24 relative, so neither the slab's rounding nor the Moeller-Trumbore t of a triangle on its box's face can cull it.
+    static constexpr float SLAB_SLACK = 16384.0f * 0x1p-24f;
     static bool slab(const BvhNode& n, const Ray& r, float3 inv_dir, float tmax) {
         float3 t0 = (n.bmin - r.origin) * inv_dir, t1 = (n.bmax - r.origin) * inv_dir;
+        // a ray lying in a box plane (0 * inf = NaN, dropped by min/max) culls the box: the padding keeps every triangle strictly inside
         float3 a = min(t0, t1), b = max(t0, t1);
         float tn = max(max(a.x, a.y), max(a.z, r.tmin)), tf = min(min(b.x, b.y), min(b.z, tmax));
-        return tn <= tf;   // NaNs (0*inf) compare false => conservative enough for axis-aligned rays exactly on a slab plane: handled by padding
+        tn = kjb_fma(-SLAB_SLACK, abs(tn), tn); tf = kjb_fma(SLAB_SLACK, abs(tf), tf);
+        return tn <= tf;
     }
     struct HitInfo { bool hit; float t, u, v; uint32_t tri; };
     HitInfo closest(const Ray& r, bool cull_back) const {
@@ -164,7 +170,7 @@ struct Scene {
             if (intersect_tri(tris[id], r, r.tmax, cull_back, t, u, v)) if (!h.hit || t < h.t || (t == h.t && id < h.tri)) { h.hit = true; h.t = t; h.u = u; h.v = v; h.tri = id; } }
         return h;
     }
-    bool any_hit(const Ray& r) const {
+    bool any_hit(const Ray& r, bool cull_back = false) const {
         n_any++;
         if (nodes.empty() || ray_has_nan(r)) return false;
         float3 inv_dir = 1.0f / r.dir;
@@ -173,7 +179,7 @@ struct Scene {
             const BvhNode& n = nodes[stack[--sp]];
             if (!slab(n, r, inv_dir, r.tmax)) continue;
             if (n.count > 0) {
-                for (int i = n.first; i < n.first + n.count; ++i) { float t, u, v; if (intersect_tri(tris[tri_order[i]], r, r.tmax, false, t, u, v)) return true; }
+                for (int i = n.first; i < n.first + n.count; ++i) { float t, u, v; if (intersect_tri(tris[tri_order[i]], r, r.tmax, cull_back, t, u, v)) return true; }
             } else { stack[sp++] = n.left; stack[sp++] = n.right; }
         }
         return false;

@@ -15,6 +15,26 @@ def make_world(lib, scene, width, height, **kw):
     return w
 
 
+def world_triangles(scene):
+    """gid-ordered (instance-major, as scenes.populate adds them) world-space triangles float32[n, 9] and tri_info uint32[n, 2], with the
+    library's xform_point: ((m0 x + m1 y) + m2 z) + m3 in float32, no contraction"""
+    tris, info, inst = [], [], 0
+    for mesh, transforms in scene:
+        p = np.asarray(mesh["positions"], np.float32)[np.asarray(mesh["indices"], np.int64)]
+        for t in transforms:
+            m = np.asarray(t, np.float32).reshape(12)
+            w = np.empty_like(p)
+            for r in range(3):
+                w[:, r] = ((m[4 * r] * p[:, 0] + m[4 * r + 1] * p[:, 1]) + m[4 * r + 2] * p[:, 2]) + m[4 * r + 3]
+            tris.append(w.reshape(-1, 9))
+            n = len(w) // 3
+            info.append(np.stack([np.full(n, inst, np.uint32), np.arange(n, dtype=np.uint32)], 1))
+            inst += 1
+    if not tris:
+        return np.zeros((0, 9), np.float32), np.zeros((0, 2), np.uint32)
+    return np.ascontiguousarray(np.concatenate(tris)), np.concatenate(info)
+
+
 def compare_images(wa, wb, names=None, rtol=0.0):
     """returns list of (name, n_mismatching_texels, max_abs_err) for images that differ"""
     bad = []
