@@ -7,67 +7,6 @@
 
 using namespace kjb;
 
-// ---- TMA tensor maps (kjb_tile.cuh).  The image is described as a 2-D tensor of 32-bit words (4-, 8- and 16-byte texels; the x
-// coordinate of a copy is scaled by words-per-texel) or of its own 1- / 2-byte elements; the box is the tile, rows padded to 16 bytes.
-namespace kjb {
-#if defined(KJB_EMU)
-TileSource tile_source(kjb_context*, const kjb_image&, uint32_t, uint32_t) { TileSource t; t.tensor_ok = 0; t.rows_ok = 0; return t; }
-int tile_mode(std::initializer_list<const TileSource*>) { return KJB_TILE_LOADS; }
-#else
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = [] {
-        void* p = nullptr; cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) p = nullptr;
-        return (EncodeTiledFn)p;
-    }();
-    return fn;
-}
-TileSource tile_source(kjb_context* c, const kjb_image& img, uint32_t box_w, uint32_t box_h) {
-    const auto key = std::make_tuple((const void*)img.data, img.width, img.height, img.format, box_w, box_h);
-    auto it = c->tile_sources.find(key);
-    if (it != c->tile_sources.end()) return it->second;
-    TileSource t; memset(&t, 0, sizeof(t));
-    const uint32_t tb = texel_bytes(img.format);
-    const uint64_t row_bytes = uint64_t(img.width) * tb;
-    EncodeTiledFn enc = encode_tiled_fn();
-    const uint32_t pitch_texels = ((box_w * tb + 15) / 16 * 16) / tb;   // == tile_pitch<tb>(box_w)
-    const uint32_t words = tb >= 4 ? tb / 4 : 1;
-    t.rows_ok = tb && (row_bytes % 16 == 0) && (uintptr_t(img.data) % 16 == 0) && img.layers <= 1;
-    if (enc && t.rows_ok && pitch_texels * words <= 256 && box_h <= 256) {
-        const CUtensorMapDataType dt = tb >= 4 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : (tb == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8);
-        const cuuint64_t dims[2] = {cuuint64_t(img.width) * words, img.height};
-        const cuuint64_t strides[1] = {row_bytes};
-        const cuuint32_t box[2] = {pitch_texels * words, box_h};
-        const cuuint32_t estr[2] = {1, 1};
-        if (enc(&t.map, dt, 2, img.data, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
-            t.tensor_ok = 1;
-    }
-    c->tile_sources[key] = t;
-    return t;
-}
-int tile_mode(std::initializer_list<const TileSource*> sources) {
-    // Preference: per-row bulk copies (UBLKCP) by default.  The tensor-map form (UTMALDG, KJB_TILE_MODE=tensor) runs bit-exact on H100 too,
-    // at the same frame time within the run-to-run spread (DESIGN §5a), so the default stays with the form the whole GPU suite runs.
-    // KJB_TILE_MODE=loads is the A/B switch.
-    static const int pref = [] {
-        const char* e = getenv("KJB_TILE_MODE"); const char* off = getenv("KJB_NO_TMA");
-        if (off && off[0] == '1') return KJB_TILE_LOADS;
-        if (e && !strcmp(e, "loads")) return KJB_TILE_LOADS;
-        if (e && !strcmp(e, "tensor")) return KJB_TILE_TMA_TENSOR;
-        return KJB_TILE_TMA_ROWS;
-    }();
-    bool tensor = true, rows = true;
-    for (const TileSource* t : sources) { tensor = tensor && t->tensor_ok; rows = rows && t->rows_ok; }
-    if (pref == KJB_TILE_TMA_TENSOR && tensor) return KJB_TILE_TMA_TENSOR;
-    if (pref != KJB_TILE_LOADS && rows) return KJB_TILE_TMA_ROWS;
-    return KJB_TILE_LOADS;
-}
-#endif
-}  // namespace kjb
-
 // ---- "rebuild tlas" on the device.  The reference rebuilds its TLAS every frame (world_renderer.rs:865-911, ray_tracing.rs:455-520); here the
 // acceleration structure is ONE flattened world-space BVH, so a transform change means new world-space triangles and new boxes.  When only
 // transforms changed (same instances, same meshes) the topology is kept and two kernels redo the rest: (1) every leaf-order triangle record
@@ -214,7 +153,6 @@ static void drop_ircache_scratch(kjb_context* c, const void* p) {
     c->ircache_scratch.erase(it);
 }
 int kjb_image_free(kjb_context* c, kjb_image* img) {
-    for (auto it = c->tile_sources.begin(); it != c->tile_sources.end();) { if (std::get<0>(it->first) == img->data) it = c->tile_sources.erase(it); else ++it; }   // the address may be reused
     drop_ircache_scratch(c, img->data);
     dev_free(img->data); img->data = nullptr; return 0;
 }

@@ -6,7 +6,6 @@
 #include "kjb_trace.cuh"
 #include "kjb_tile.cuh"
 #include <map>
-#include <tuple>
 #include <initializer_list>
 #include <string>
 #include <vector>
@@ -68,8 +67,6 @@ struct kjb_context {
 #endif
     uint64_t graph_launches = 0, graph_instantiations = 0;
     kjb::Globals g;   // host copy, passed by value to every kernel
-    // tensor maps of the images the tiled kernels stage through TMA, one per (image, box): built on first use, dropped when the image is freed
-    std::map<std::tuple<const void*, uint32_t, uint32_t, uint32_t, uint32_t, uint32_t>, kjb::TileSource> tile_sources;
     // device scratch of the irradiance cache's ordered schedule (kjb_ircache.cuh), one set per cache, keyed by its life_buf; freed with that buffer
     struct IrcacheScratch { void* claim_rank; void* claim_vertex; void* life_pending; void* scan; void* claim_bits; void* aux_prev; void* entry_vertex; };
     std::map<const void*, IrcacheScratch> ircache_scratch;
@@ -137,13 +134,6 @@ inline int dev_sync(kjb_context* c) {   // every queue of the context
 inline const char* dev_check(kjb_context*) { cudaError_t e = cudaGetLastError(); return e == cudaSuccess ? nullptr : cudaGetErrorString(e); }
 #endif
 
-inline uint32_t texel_bytes(uint32_t f);
-// TileSource of `img` for tiles of box_w x box_h texels (kjb_tile.cuh).  use_tma = 0 when the image cannot be described to the copy engine
-// (row pitch or base not 16-byte aligned, driver entry point missing): the kernels then stage the same tile with guarded loads.
-kjb::TileSource tile_source(kjb_context* c, const kjb_image& img, uint32_t box_w, uint32_t box_h);
-// staging mode of one launch (KJB_TILE_*): what every source of the launch supports, under the process-wide preference KJB_TILE_MODE = rows | tensor | loads
-int tile_mode(std::initializer_list<const kjb::TileSource*> sources);
-
 inline uint32_t texel_bytes(uint32_t f) {
     switch (f) {
         case KJB_FMT_R32_FLOAT: case KJB_FMT_RG16_FLOAT: case KJB_FMT_RGBA8_UNORM: case KJB_FMT_RGBA8_SNORM:
@@ -156,6 +146,18 @@ inline uint32_t texel_bytes(uint32_t f) {
     }
 }
 inline size_t image_bytes(const kjb_image& i) { return size_t(i.width) * i.height * (i.layers ? i.layers : 1) * texel_bytes(i.format); }
+
+// staging form of one tiled launch (kjb_tile.cuh): row bulk copies when every staged image has a 16-byte aligned base and row pitch and one
+// layer, guarded loads otherwise and always in the CPU emulator
+inline int tile_mode(std::initializer_list<const kjb_image*> imgs) {
+#if defined(KJB_EMU)
+    (void)imgs; return KJB_TILE_LOADS;
+#else
+    for (const kjb_image* i : imgs)
+        if (!texel_bytes(i->format) || uint64_t(i->width) * texel_bytes(i->format) % 16 || uintptr_t(i->data) % 16 || i->layers > 1) return KJB_TILE_LOADS;
+    return KJB_TILE_ROWS;
+#endif
+}
 
 // argument validation shared by all pass entry points: format + non-null + (optionally) extent
 inline bool check_img(kjb_context* c, const kjb_image& i, uint32_t fmt, const char* pass, const char* name, uint32_t w = 0, uint32_t h = 0) {
@@ -187,7 +189,7 @@ inline bool check_img(kjb_context* c, const kjb_image& i, uint32_t fmt, const ch
 #define KJB_DIMS(...) __VA_ARGS__
 // Ray-tracing passes: 8 x 16 pixel blocks, so that a warp (32 consecutive threads) is an 8 x 4 pixel patch — compact footprints keep the
 // lanes of a warp on neighbouring BVH nodes and make hit / miss shading branch together more often than 32 x 1 or 16 x 2 strips.  The
-// serial twins (and the oracle's serial schedule, oracle/kj_ctx.h) walk the pixels in the same block order.
+// serial schedule (KJB_PIXELS below, and the oracle's, oracle/kj_ctx.h) walks the pixels in the same block order.
 #ifndef KJB_RAY_BX
 #define KJB_RAY_BX 8
 #endif
@@ -198,5 +200,25 @@ inline bool check_img(kjb_context* c, const kjb_image& i, uint32_t fmt, const ch
 #define KJB_ROWS(ctx, H) const kjb::Rows kjb__rows = (ctx)->rows_for(H)
 #define KJB_GRID2D(W, H, BX, BY) dim3(((W) + (BX) - 1) / (BX), (unsigned(kjb__rows.y1 - kjb__rows.y0) + (BY) - 1) / (BY), 1), dim3((BX), (BY), 1)
 #define KJB_PX int x = int(blockIdx.x * blockDim.x + threadIdx.x), y = kjb_rows.y0 + int(blockIdx.y * blockDim.y + threadIdx.y); if (y >= kjb_rows.y1) return
+
+// Serial schedule (kjb_set_debug_serial): a kernel that touches the irradiance cache is a `template <bool SERIAL>`; its `<true>` form runs
+// on thread 0 of one block and walks the logical threads of the parallel launch in launch order — the deterministic schedule of the CPU
+// oracle, so that the racy cache passes compare bit for bit on the GPU (slow; a test / repro aid only).  `__VA_ARGS__` is the per-thread work.
+// Pixel grid: the pixel (x, y) of this thread in a W x H grid — or, SERIAL, every pixel: KJB_RAY_BX x KJB_RAY_BY blocks row-major over the
+// rows of the launch, pixels row-major inside a block (the oracle's order, oracle/kj_ctx.h).
+#define KJB_PIXELS(SERIAL, W, H, ...) do { \
+        if constexpr (SERIAL) { \
+            if (blockIdx.x | blockIdx.y | threadIdx.x | threadIdx.y) return; \
+            for (int by = kjb_rows.y0; by < kjb_rows.y1; by += KJB_RAY_BY) for (int bx = 0; bx < (W); bx += KJB_RAY_BX) \
+                for (int y = by; y < by + KJB_RAY_BY && y < kjb_rows.y1 && y < (H); ++y) for (int x = bx; x < bx + KJB_RAY_BX && x < (W); ++x) { __VA_ARGS__; } \
+        } else { KJB_PX; if (x >= (W) || y >= (H)) return; __VA_ARGS__; } } while (0)
+// 1-D, the serial form only: logical threads i = 0 .. n-1 in order
+#define KJB_SERIAL_1D(n, ...) do { if (blockIdx.x | threadIdx.x) return; for (uint32_t i = 0, n__ = (n); i < n__; ++i) { __VA_ARGS__; } } while (0)
+// Launch of such a kernel: `kernel<true>` on one block under the serial schedule, else `kernel<false>` with `dims` — as an ordered launch
+// while `bound` (the pass touches a bound cache), as a plain one otherwise
+#define KJB_LAUNCH_CACHE(ctx, bound, kernel, dims, ...) do { \
+        if ((bound) && (ctx)->debug_serial) KJB_LAUNCH(ctx, kernel<true>, KJB_DIMS(dim3(1), dim3(32)), __VA_ARGS__); \
+        else if (bound) KJB_LAUNCH_ORDERED(ctx, kernel<false>, KJB_DIMS(dims), __VA_ARGS__); \
+        else KJB_LAUNCH(ctx, kernel<false>, KJB_DIMS(dims), __VA_ARGS__); } while (0)
 
 #define KJB_PASS_EPILOGUE(ctx, name) do { const char* e__ = kjb::dev_check(ctx); if (e__) return (ctx)->fail(std::string(name) + ": " + e__); return 0; } while (0)

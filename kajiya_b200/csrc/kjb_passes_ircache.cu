@@ -50,15 +50,13 @@ KJB_DEV void ircache_scroll_cell(const Globals& g, const uint32_t* gm, uint32_t*
         if (m1 & IRCACHE_ENTRY_META_OCCUPIED) entry_cell[m0] = dst_cell_idx;
     } else { gm2[dst_cell_idx * 2] = 0; gm2[dst_cell_idx * 2 + 1] = 0; }
 }
+// SERIAL (here and in the age, validate and trace passes): ONE thread walks the logical threads in launch order — the serial schedule
+// (kjb_set_debug_serial, KJB_SERIAL_1D in kjb_context.h); the ordered schedule's scratch is never attached under it (`parallel` = 0)
+template <bool SERIAL>
 KJB_KERNEL(256) k_ircache_scroll_cascades(const __grid_constant__ Globals g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta,
                                           uint32_t parallel, Rows kjb_rows) {
-    const uint32_t i = tid1d(); if (i < KJB_IRCACHE_GRID_CELLS) ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i, parallel != 0);
-}
-// `_serial` twins (kjb_set_debug_serial): ONE thread walks the logical threads in launch order — the deterministic schedule the
-// CPU oracle uses, so the racy cache passes can be compared bit for bit on the real GPU (slow; test / repro aid only)
-KJB_KERNEL(32) k_ircache_scroll_cascades_serial(const __grid_constant__ Globals g, const uint32_t* gm, uint32_t* gm2, uint32_t* entry_cell, float4* irradiance, uint32_t* life, uint32_t* pool, uint32_t* meta, Rows kjb_rows) {
-    if (tid1d() != 0) return;
-    for (uint32_t i = 0; i < KJB_IRCACHE_GRID_CELLS; ++i) ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i);
+    if constexpr (SERIAL) KJB_SERIAL_1D(KJB_IRCACHE_GRID_CELLS, ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i, parallel != 0));
+    else { const uint32_t i = tid1d(); if (i < KJB_IRCACHE_GRID_CELLS) ircache_scroll_cell(g, gm, gm2, entry_cell, irradiance, life, pool, meta, i, parallel != 0); }
 }
 
 // ------------------------------------------------------------------ I3 prepare_age_dispatch_args.hlsl / prepare_trace_dispatch_args.hlsl
@@ -111,14 +109,11 @@ KJB_DEV void ircache_age_entry(uint32_t* meta, uint32_t* gm, uint32_t* entry_cel
     const uint32_t l2 = life[entry_idx];
     occupancy[entry_idx] = (entry_idx < total_entry_count && is_ircache_entry_life_valid(l2)) ? 1u : 0u;
 }
+template <bool SERIAL>
 KJB_KERNEL(256) k_ircache_age(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, uint32_t* pool, float4* spatial, float4* proposal, uint32_t* proposal_count,
                               float4* irradiance, uint32_t* occupancy, float4* entry_vertex, Rows kjb_rows) {
-    const uint32_t i = tid1d(); if (i < MAX_ENTRIES) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i, entry_vertex);
-}
-KJB_KERNEL(32) k_ircache_age_serial(uint32_t* meta, uint32_t* gm, uint32_t* entry_cell, uint32_t* life, uint32_t* pool, float4* spatial, float4* proposal, uint32_t* proposal_count,
-                                    float4* irradiance, uint32_t* occupancy, Rows kjb_rows) {
-    if (tid1d() != 0) return;
-    for (uint32_t i = 0; i < MAX_ENTRIES; ++i) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i);
+    if constexpr (SERIAL) KJB_SERIAL_1D(MAX_ENTRIES, ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i, entry_vertex));
+    else { const uint32_t i = tid1d(); if (i < MAX_ENTRIES) ircache_age_entry(meta, gm, entry_cell, life, pool, spatial, proposal, proposal_count, irradiance, occupancy, i, entry_vertex); }
 }
 
 // ------------------------------------------------------------------ the parallel schedule's entry assignment (kjb_ircache.cuh), at the start of a chain
@@ -372,11 +367,13 @@ KJB_DEV void ircache_validate_sample(const Globals& g, const IrcacheBufs& b, con
         b.aux[output_idx + IRCACHE_OCTA_DIMS2] = prev_value_and_count;
     }
 }
-KJB_KERNEL(128) k_ircache_validate(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) { ircache_validate_sample(g, b, sky_cube_tex, indirection, tid1d()); }
-KJB_KERNEL(32) k_ircache_validate_serial(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) {
-    if (tid1d() != 0) return;
-    const uint32_t n = b.meta[IRCACHE_META_TRACING_ALLOC_COUNT] * IRCACHE_VALIDATION_SAMPLES_PER_FRAME;
-    for (uint32_t i = 0; i < n && i < MAX_ENTRIES * IRCACHE_VALIDATION_SAMPLES_PER_FRAME; ++i) ircache_validate_sample(g, b, sky_cube_tex, indirection, i);
+// the serial form (as k_ircache_trace's) walks the samples of the traced entries only: the parallel launch's threads beyond them return at once
+template <bool SERIAL>
+KJB_KERNEL(128) k_ircache_validate(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) {
+    if constexpr (SERIAL) {
+        const uint32_t n = b.meta[IRCACHE_META_TRACING_ALLOC_COUNT] * IRCACHE_VALIDATION_SAMPLES_PER_FRAME, n_max = MAX_ENTRIES * IRCACHE_VALIDATION_SAMPLES_PER_FRAME;
+        KJB_SERIAL_1D(n < n_max ? n : n_max, ircache_validate_sample(g, b, sky_cube_tex, indirection, i));
+    } else ircache_validate_sample(g, b, sky_cube_tex, indirection, tid1d());
 }
 
 // ------------------------------------------------------------------ I10 trace_irradiance.rgen.hlsl:44-145
@@ -413,11 +410,12 @@ KJB_DEV void ircache_trace_sample(const Globals& g, const IrcacheBufs& b, const 
     b.aux[output_idx + IRCACHE_OCTA_DIMS2] = f4(val_sel, reservoir.W);
     if (selected_new) b.aux[output_idx + IRCACHE_OCTA_DIMS2 * 2] = packed_entry;
 }
-KJB_KERNEL(128) k_ircache_trace(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) { ircache_trace_sample(g, b, sky_cube_tex, indirection, tid1d()); }
-KJB_KERNEL(32) k_ircache_trace_serial(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) {
-    if (tid1d() != 0) return;
-    const uint32_t n = b.meta[IRCACHE_META_TRACING_ALLOC_COUNT] * IRCACHE_SAMPLES_PER_FRAME;
-    for (uint32_t i = 0; i < n && i < MAX_ENTRIES * IRCACHE_SAMPLES_PER_FRAME; ++i) ircache_trace_sample(g, b, sky_cube_tex, indirection, i);
+template <bool SERIAL>
+KJB_KERNEL(128) k_ircache_trace(const __grid_constant__ Globals g, IrcacheBufs b, Img sky_cube_tex, const uint32_t* indirection, Rows kjb_rows) {
+    if constexpr (SERIAL) {
+        const uint32_t n = b.meta[IRCACHE_META_TRACING_ALLOC_COUNT] * IRCACHE_SAMPLES_PER_FRAME, n_max = MAX_ENTRIES * IRCACHE_SAMPLES_PER_FRAME;
+        KJB_SERIAL_1D(n < n_max ? n : n_max, ircache_trace_sample(g, b, sky_cube_tex, indirection, i));
+    } else ircache_trace_sample(g, b, sky_cube_tex, indirection, tid1d());
 }
 
 // ------------------------------------------------------------------ I11 sum_up_irradiance.hlsl:34-89
@@ -548,10 +546,8 @@ int kjb_pass_ircache_scroll_cascades(kjb_context* c, const kjb_ircache_scroll_ca
         KJB_LAUNCH(c, k_ircache_det_assign, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), (const uint32_t*)U32P(a->pool_buf),
                    (float4*)s.entry_vertex, (uint32_t*)s.claim_rank, (float4*)s.claim_vertex, (const uint32_t*)free_scan, (const uint32_t*)s.claim_bits, (const uint32_t*)claim_scan);
     }
-    if (c->debug_serial) KJB_LAUNCH(c, k_ircache_scroll_cascades_serial, DIMS1D(1, 32), c->g, U32P(a->grid_meta_buf), U32P(a->grid_meta_buf2), U32P(a->entry_cell_buf), F4P(a->irradiance_buf),
-                       U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf));
-    else KJB_LAUNCH_ORDERED(c, k_ircache_scroll_cascades, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), c->g, U32P(a->grid_meta_buf), U32P(a->grid_meta_buf2), U32P(a->entry_cell_buf), F4P(a->irradiance_buf),
-                       U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf), ircache_parallel_scratch(c, a->life_buf.data, s) ? 1u : 0u);
+    KJB_LAUNCH_CACHE(c, true, k_ircache_scroll_cascades, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), c->g, U32P(a->grid_meta_buf), U32P(a->grid_meta_buf2), U32P(a->entry_cell_buf), F4P(a->irradiance_buf),
+                     U32P(a->life_buf), U32P(a->pool_buf), U32P(a->meta_buf), ircache_parallel_scratch(c, a->life_buf.data, s) ? 1u : 0u);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_ircache_prepare_age_dispatch_args(kjb_context* c, const kjb_ircache_dispatch_args_args* a) {
@@ -573,14 +569,10 @@ int kjb_pass_ircache_age_entries(kjb_context* c, const kjb_ircache_age_args* a) 
     BUF(a->reposition_proposal_buf, float4, MAX_ENTRIES, "reposition_proposal_buf"); BUF(a->reposition_proposal_count_buf, uint32_t, MAX_ENTRIES, "reposition_proposal_count_buf");
     BUF(a->irradiance_buf, float4, 3 * MAX_ENTRIES, "irradiance_buf"); BUF(a->entry_occupancy_buf, uint32_t, MAX_ENTRIES, "entry_occupancy_buf");
     NO_SCISSOR;
-    if (c->debug_serial) KJB_LAUNCH(c, k_ircache_age_serial, DIMS1D(1, 32), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
-                       F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf));
-    else {
-        kjb_context::IrcacheScratch s;
-        float4* entry_vertex = ircache_parallel_scratch(c, a->life_buf.data, s) ? (float4*)s.entry_vertex : nullptr;
-        KJB_LAUNCH_ORDERED(c, k_ircache_age, DIMS1D(MAX_ENTRIES, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
-                           F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf), entry_vertex);
-    }
+    kjb_context::IrcacheScratch s;
+    float4* entry_vertex = ircache_parallel_scratch(c, a->life_buf.data, s) ? (float4*)s.entry_vertex : nullptr;
+    KJB_LAUNCH_CACHE(c, true, k_ircache_age, DIMS1D(MAX_ENTRIES, 256), U32P(a->meta_buf), U32P(a->grid_meta_buf), U32P(a->entry_cell_buf), U32P(a->life_buf), U32P(a->pool_buf), F4P(a->spatial_buf),
+                     F4P(a->reposition_proposal_buf), U32P(a->reposition_proposal_count_buf), F4P(a->irradiance_buf), U32P(a->entry_occupancy_buf), entry_vertex);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_inclusive_prefix_scan_u32(kjb_context* c, const kjb_prefix_scan_args* a) {
@@ -635,16 +627,14 @@ int kjb_pass_ircache_validate(kjb_context* c, const kjb_ircache_trace_args* a) {
     const char* P = "ircache validate"; IrcacheBufs b; if (check_trace_args(c, P, a, b)) return 1;
     snapshot_aux(c, b);
     NO_SCISSOR;
-    if (c->debug_serial) KJB_LAUNCH(c, k_ircache_validate_serial, DIMS1D(1, 32), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
-    else KJB_LAUNCH_ORDERED(c, k_ircache_validate, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
+    KJB_LAUNCH_CACHE(c, true, k_ircache_validate, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_ircache_trace(kjb_context* c, const kjb_ircache_trace_args* a) {
     const char* P = "ircache trace"; IrcacheBufs b; if (check_trace_args(c, P, a, b)) return 1;
     snapshot_aux(c, b);
     NO_SCISSOR;
-    if (c->debug_serial) KJB_LAUNCH(c, k_ircache_trace_serial, DIMS1D(1, 32), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
-    else KJB_LAUNCH_ORDERED(c, k_ircache_trace, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
+    KJB_LAUNCH_CACHE(c, true, k_ircache_trace, DIMS1D(MAX_ENTRIES * 4u, 128), c->g, b, img_ro(a->sky_cube_tex), U32P(a->entry_indirection_buf));
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_ircache_sum(kjb_context* c, const kjb_ircache_sum_args* a) {

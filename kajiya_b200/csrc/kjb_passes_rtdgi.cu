@@ -183,20 +183,11 @@ KJB_DEV void rtdgi_validate_px(const Globals& g, const Img& half_view_normal_tex
 #ifndef KJB_OCC_VALIDATE
 #define KJB_OCC_VALIDATE 8   /* 64 registers */
 #endif
+template <bool SERIAL>   // SERIAL: the serial schedule's form (KJB_PIXELS, kjb_context.h)
 KJB_KERNEL_OCC(128, KJB_OCC_VALIDATE) k_rtdgi_validate(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, ImgW reservoir_tex, Img reservoir_ray_history_tex,
                                  Img sky_cube_tex, ImgW irradiance_history_tex, Img ray_orig_history_tex, ImgW out_tex, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_PX; if (x >= out_tex.w || y >= out_tex.h) return;
-    rtdgi_validate_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reservoir_tex, reservoir_ray_history_tex, sky_cube_tex, irradiance_history_tex, ray_orig_history_tex, out_tex, gts, ircache, x, y);
-}
-// `_serial` twins (kjb_set_debug_serial, see kjb_passes_ircache.cu): one thread walks the pixels in the launch order of the
-// parallel kernel — 8x16 blocks row-major, pixels row-major inside a block
-#define KJB_SERIAL_TILES(W, H, ...) do { if (blockIdx.x | blockIdx.y | threadIdx.x | threadIdx.y) return; \
-        for (int by = kjb_rows.y0; by < kjb_rows.y1; by += KJB_RAY_BY) for (int bx = 0; bx < (W); bx += KJB_RAY_BX) \
-            for (int y = by; y < by + KJB_RAY_BY && y < kjb_rows.y1 && y < (H); ++y) for (int x = bx; x < bx + KJB_RAY_BX && x < (W); ++x) { __VA_ARGS__; } } while (0)
-KJB_KERNEL(32) k_rtdgi_validate_serial(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, ImgW reservoir_tex, Img reservoir_ray_history_tex,
-                                       Img sky_cube_tex, ImgW irradiance_history_tex, Img ray_orig_history_tex, ImgW out_tex, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_SERIAL_TILES(out_tex.w, out_tex.h, rtdgi_validate_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reservoir_tex, reservoir_ray_history_tex, sky_cube_tex, irradiance_history_tex,
-                                                              ray_orig_history_tex, out_tex, gts, ircache, x, y));
+    KJB_PIXELS(SERIAL, out_tex.w, out_tex.h, rtdgi_validate_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reservoir_tex, reservoir_ray_history_tex, sky_cube_tex, irradiance_history_tex,
+                                                                ray_orig_history_tex, out_tex, gts, ircache, x, y));
 }
 
 // ------------------------------------------------------------------ D4 trace_diffuse.rgen.hlsl:49-120
@@ -237,14 +228,10 @@ KJB_DEV void rtdgi_trace_px(const Globals& g, const Img& half_view_normal_tex, c
 #ifndef KJB_OCC_TRACE
 #define KJB_OCC_TRACE 8   /* 64 registers */
 #endif
+template <bool SERIAL>
 KJB_KERNEL_OCC(128, KJB_OCC_TRACE) k_rtdgi_trace(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, Img reprojection_tex, Img sky_cube_tex,
                               ImgW cand_irr, ImgW cand_normal, ImgW cand_hit, Img inv_in, ImgW inv_out, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_PX; if (x >= cand_irr.w || y >= cand_irr.h) return;
-    rtdgi_trace_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reprojection_tex, sky_cube_tex, cand_irr, cand_normal, cand_hit, inv_in, inv_out, gts, ircache, x, y);
-}
-KJB_KERNEL(32) k_rtdgi_trace_serial(const __grid_constant__ Globals g, Img half_view_normal_tex, Img depth_tex, Img reprojected_gi_tex, Img reprojection_tex, Img sky_cube_tex,
-                                    ImgW cand_irr, ImgW cand_normal, ImgW cand_hit, Img inv_in, ImgW inv_out, float4 gts, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_SERIAL_TILES(cand_irr.w, cand_irr.h, rtdgi_trace_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reprojection_tex, sky_cube_tex, cand_irr, cand_normal, cand_hit, inv_in, inv_out, gts, ircache, x, y));
+    KJB_PIXELS(SERIAL, cand_irr.w, cand_irr.h, rtdgi_trace_px(g, half_view_normal_tex, depth_tex, reprojected_gi_tex, reprojection_tex, sky_cube_tex, cand_irr, cand_normal, cand_hit, inv_in, inv_out, gts, ircache, x, y));
 }
 
 // ------------------------------------------------------------------ D5 temporal_validity_integrate.hlsl:21-119
@@ -736,7 +723,7 @@ struct Weights25 { float w[25]; float w_sum; };   // w_sum: the float sum of w[]
 #define D10_BY 16
 #define D10_TW (D10_BX + 4)
 #define D10_TH (D10_BY + 4)
-KJB_KERNEL(512) k_rtdgi_temporal(const __grid_constant__ TileSource ts_input, const __grid_constant__ TileSource ts_history, int tile_mode_, Globals g, Img input_tex, Img history_tex,
+KJB_KERNEL(512) k_rtdgi_temporal(int tile_mode_, Globals g, Img input_tex, Img history_tex,
                                  Img variance_history_tex, Img reprojection_tex, Img rt_history_invalidity_tex,
                                  ImgW output_tex, ImgW history_output_tex, ImgW variance_history_output_tex, float4 ots, Weights25 wt, Rows kjb_rows) {
     constexpr int PR = tile_pitch<8>(D10_TW);
@@ -751,8 +738,8 @@ KJB_KERNEL(512) k_rtdgi_temporal(const __grid_constant__ TileSource ts_input, co
     const float4 history_mult = f4(ped, ped, ped, 1);
     const int tid = int(threadIdx.y) * D10_BX + int(threadIdx.x);
     tile_group_begin(&bar, 0, tile_mode_, tid);
-    uint32_t staged = tile_issue<uint2, D10_TW, D10_TH>(s_raw_in, ts_input, input_tex, bx0, by0, &bar, tile_mode_, tid, D10_BX * D10_BY);
-    staged += tile_issue<uint2, D10_TW, D10_TH>(s_raw_hist, ts_history, history_tex, bx0, by0, &bar, tile_mode_, tid, D10_BX * D10_BY);
+    uint32_t staged = tile_issue<uint2, D10_TW, D10_TH>(s_raw_in, input_tex, bx0, by0, &bar, tile_mode_, tid, D10_BX * D10_BY);
+    staged += tile_issue<uint2, D10_TW, D10_TH>(s_raw_hist, history_tex, bx0, by0, &bar, tile_mode_, tid, D10_BX * D10_BY);
     tile_group_wait(&bar, 0, tile_mode_, staged, tid);
     for (int i = tid; i < D10_TW * D10_TH; i += D10_BX * D10_BY) {
         const int tx = i % D10_TW, ty = i / D10_TW;
@@ -881,15 +868,9 @@ int kjb_pass_rtdgi_validate(kjb_context* c, const kjb_rtdgi_validate_args* a) {
     CHKE(a->irradiance_history_tex, KJB_FMT_RGBA16_FLOAT, "irradiance_history_tex", W, H); CHKE(a->ray_orig_history_tex, KJB_FMT_RGBA32_FLOAT, "ray_orig_history_tex", W, H);
     IrcacheBufs ircache; if (check_ircache_bindings(c, P, a->ircache, ircache)) return 1;
     KJB_ROWS(c, H);
-    if (ircache.bound() && c->debug_serial)
-        KJB_LAUNCH(c, k_rtdgi_validate_serial, KJB_DIMS(dim3(1), dim3(32)), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_rw(a->reservoir_tex),
-               img_ro(a->reservoir_ray_history_tex), img_ro(a->sky_cube_tex), img_rw(a->irradiance_history_tex), img_ro(a->ray_orig_history_tex), img_rw(a->rt_history_invalidity_out_tex), F4A(a->gbuffer_tex_size), ircache);
-    else if (ircache.bound())
-        KJB_LAUNCH_ORDERED(c, k_rtdgi_validate, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_rw(a->reservoir_tex),
-               img_ro(a->reservoir_ray_history_tex), img_ro(a->sky_cube_tex), img_rw(a->irradiance_history_tex), img_ro(a->ray_orig_history_tex), img_rw(a->rt_history_invalidity_out_tex), F4A(a->gbuffer_tex_size), ircache);
-    else
-        KJB_LAUNCH(c, k_rtdgi_validate, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_rw(a->reservoir_tex),
-               img_ro(a->reservoir_ray_history_tex), img_ro(a->sky_cube_tex), img_rw(a->irradiance_history_tex), img_ro(a->ray_orig_history_tex), img_rw(a->rt_history_invalidity_out_tex), F4A(a->gbuffer_tex_size), ircache);
+    KJB_LAUNCH_CACHE(c, ircache.bound(), k_rtdgi_validate, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex),
+                     img_rw(a->reservoir_tex), img_ro(a->reservoir_ray_history_tex), img_ro(a->sky_cube_tex), img_rw(a->irradiance_history_tex), img_ro(a->ray_orig_history_tex),
+                     img_rw(a->rt_history_invalidity_out_tex), F4A(a->gbuffer_tex_size), ircache);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_rtdgi_trace(kjb_context* c, const kjb_rtdgi_trace_args* a) {
@@ -901,18 +882,9 @@ int kjb_pass_rtdgi_trace(kjb_context* c, const kjb_rtdgi_trace_args* a) {
     CHKE(a->rt_history_invalidity_out_tex, KJB_FMT_R8_UNORM, "rt_history_invalidity_out_tex", W, H);
     IrcacheBufs ircache; if (check_ircache_bindings(c, P, a->ircache, ircache)) return 1;
     KJB_ROWS(c, H);
-    if (ircache.bound() && c->debug_serial)
-        KJB_LAUNCH(c, k_rtdgi_trace_serial, KJB_DIMS(dim3(1), dim3(32)), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_ro(a->reprojection_tex), img_ro(a->sky_cube_tex),
-               img_rw(a->candidate_irradiance_out_tex), img_rw(a->candidate_normal_out_tex), img_rw(a->candidate_hit_out_tex), img_ro(a->rt_history_invalidity_in_tex), img_rw(a->rt_history_invalidity_out_tex),
-               F4A(a->gbuffer_tex_size), ircache);
-    else if (ircache.bound())
-        KJB_LAUNCH_ORDERED(c, k_rtdgi_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_ro(a->reprojection_tex), img_ro(a->sky_cube_tex),
-               img_rw(a->candidate_irradiance_out_tex), img_rw(a->candidate_normal_out_tex), img_rw(a->candidate_hit_out_tex), img_ro(a->rt_history_invalidity_in_tex), img_rw(a->rt_history_invalidity_out_tex),
-               F4A(a->gbuffer_tex_size), ircache);
-    else
-        KJB_LAUNCH(c, k_rtdgi_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex), img_ro(a->reprojection_tex), img_ro(a->sky_cube_tex),
-               img_rw(a->candidate_irradiance_out_tex), img_rw(a->candidate_normal_out_tex), img_rw(a->candidate_hit_out_tex), img_ro(a->rt_history_invalidity_in_tex), img_rw(a->rt_history_invalidity_out_tex),
-               F4A(a->gbuffer_tex_size), ircache);
+    KJB_LAUNCH_CACHE(c, ircache.bound(), k_rtdgi_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, img_ro(a->half_view_normal_tex), img_ro(a->depth_tex), img_ro(a->reprojected_gi_tex),
+                     img_ro(a->reprojection_tex), img_ro(a->sky_cube_tex), img_rw(a->candidate_irradiance_out_tex), img_rw(a->candidate_normal_out_tex), img_rw(a->candidate_hit_out_tex),
+                     img_ro(a->rt_history_invalidity_in_tex), img_rw(a->rt_history_invalidity_out_tex), F4A(a->gbuffer_tex_size), ircache);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_rtdgi_validity_integrate(kjb_context* c, const kjb_rtdgi_validity_integrate_args* a) {
@@ -1012,8 +984,7 @@ int kjb_pass_rtdgi_temporal(kjb_context* c, const kjb_rtdgi_temporal_args* a) {
     for (int yy = -2; yy <= 2; ++yy) for (int xx = -2; xx <= 2; ++xx) wt.w[(yy + 2) * 5 + (xx + 2)] = kjb_exp(-3.0f * float(xx * xx + yy * yy) / float((2 + 1.) * (2 + 1.)));
     wt.w_sum = 0; for (int i = 0; i < 25; ++i) wt.w_sum += wt.w[i];
     KJB_ROWS(c, H);
-    const TileSource ts_in = tile_source(c, a->input_tex, D10_TW, D10_TH), ts_hist = tile_source(c, a->history_tex, D10_TW, D10_TH);
-    KJB_LAUNCH_SYNC(c, k_rtdgi_temporal, KJB_GRID2D(W, H, D10_BX, D10_BY), ts_in, ts_hist, tile_mode({&ts_in, &ts_hist}), c->g, img_ro(a->input_tex), img_ro(a->history_tex), img_ro(a->variance_history_tex), img_ro(a->reprojection_tex), img_ro(a->rt_history_invalidity_tex),
+    KJB_LAUNCH_SYNC(c, k_rtdgi_temporal, KJB_GRID2D(W, H, D10_BX, D10_BY), tile_mode({&a->input_tex, &a->history_tex}), c->g, img_ro(a->input_tex), img_ro(a->history_tex), img_ro(a->variance_history_tex), img_ro(a->reprojection_tex), img_ro(a->rt_history_invalidity_tex),
                img_rw(a->output_tex), img_rw(a->history_output_tex), img_rw(a->variance_history_output_tex), F4A(a->output_tex_size), wt);
     KJB_PASS_EPILOGUE(c, P);
 }

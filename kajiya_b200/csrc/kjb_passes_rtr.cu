@@ -169,15 +169,9 @@ KJB_DEV void rtr_trace_px(const Globals& g, const RtrTraceImgs& t, const BlueNoi
 #ifndef KJB_OCC_RTR_TRACE
 #define KJB_OCC_RTR_TRACE 8   /* 80 -> 64 registers */
 #endif
+template <bool SERIAL>   // SERIAL: the serial schedule's form (KJB_PIXELS, kjb_context.h)
 KJB_KERNEL_OCC(128, KJB_OCC_RTR_TRACE) k_rtr_trace(const __grid_constant__ Globals g, RtrTraceImgs t, BlueNoiseSamplerTables bn, float4 gts, uint32_t reuse_rtdgi_rays, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_PX; if (x >= t.out0_tex.w || y >= t.out0_tex.h) return;
-    rtr_trace_px(g, t, bn, gts, reuse_rtdgi_rays, ircache, x, y);
-}
-#define KJB_SERIAL_TILES(W, H, ...) do { if (blockIdx.x | blockIdx.y | threadIdx.x | threadIdx.y) return; \
-        for (int by = kjb_rows.y0; by < kjb_rows.y1; by += KJB_RAY_BY) for (int bx = 0; bx < (W); bx += KJB_RAY_BX) \
-            for (int y = by; y < by + KJB_RAY_BY && y < kjb_rows.y1 && y < (H); ++y) for (int x = bx; x < bx + KJB_RAY_BX && x < (W); ++x) { __VA_ARGS__; } } while (0)
-KJB_KERNEL(32) k_rtr_trace_serial(const __grid_constant__ Globals g, RtrTraceImgs t, BlueNoiseSamplerTables bn, float4 gts, uint32_t reuse_rtdgi_rays, IrcacheBufs ircache, Rows kjb_rows) {
-    KJB_SERIAL_TILES(t.out0_tex.w, t.out0_tex.h, rtr_trace_px(g, t, bn, gts, reuse_rtdgi_rays, ircache, x, y));
+    KJB_PIXELS(SERIAL, t.out0_tex.w, t.out0_tex.h, rtr_trace_px(g, t, bn, gts, reuse_rtdgi_rays, ircache, x, y));
 }
 
 // ------------------------------------------------------------------ R2 reflection_validate.rgen.hlsl:42-146 (one thread per 2x2 quad of half-res pixels)
@@ -227,12 +221,9 @@ KJB_DEV void rtr_validate_quad(const Globals& g, const RtrValidateImgs& t, float
 #ifndef KJB_OCC_RTR_VALIDATE
 #define KJB_OCC_RTR_VALIDATE 8
 #endif
+template <bool SERIAL>
 KJB_KERNEL_OCC(128, KJB_OCC_RTR_VALIDATE) k_rtr_validate(const __grid_constant__ Globals g, RtrValidateImgs t, float4 gts, IrcacheBufs ircache, int QW, int QH, Rows kjb_rows) {
-    KJB_PX; if (x >= QW || y >= QH) return;
-    rtr_validate_quad(g, t, gts, ircache, x, y);
-}
-KJB_KERNEL(32) k_rtr_validate_serial(const __grid_constant__ Globals g, RtrValidateImgs t, float4 gts, IrcacheBufs ircache, int QW, int QH, Rows kjb_rows) {
-    KJB_SERIAL_TILES(QW, QH, rtr_validate_quad(g, t, gts, ircache, x, y));
+    KJB_PIXELS(SERIAL, QW, QH, rtr_validate_quad(g, t, gts, ircache, x, y));
 }
 
 // ------------------------------------------------------------------ R3 rtr_restir_temporal.hlsl:148-533
@@ -570,7 +561,7 @@ struct RtrTemporalImgs { Img input_tex, history_tex, depth_tex, ray_len_tex, rep
 #define R5_AX 4
 #define R5_LW 34
 #define R5_TH 10
-KJB_KERNEL_OCC(256, KJB_OCC_RTR_TEMPORAL) k_rtr_temporal(const __grid_constant__ TileSource ts_input, const __grid_constant__ TileSource ts_depth, int tile_mode_, Globals g, RtrTemporalImgs t, float4 ots, Rows kjb_rows) {
+KJB_KERNEL_OCC(256, KJB_OCC_RTR_TEMPORAL) k_rtr_temporal(int tile_mode_, Globals g, RtrTemporalImgs t, float4 ots, Rows kjb_rows) {
     constexpr int P4 = tile_pitch<4>(R5_TW);
     __shared__ __align__(128) uint32_t s_raw[P4 * R5_TH];
     __shared__ __align__(128) float s_depth[P4 * R5_TH];
@@ -579,8 +570,8 @@ KJB_KERNEL_OCC(256, KJB_OCC_RTR_TEMPORAL) k_rtr_temporal(const __grid_constant__
     const int tid = int(threadIdx.y) * 32 + int(threadIdx.x);
     const int bx0 = int(blockIdx.x) * 32, by0 = kjb_rows.y0 + int(blockIdx.y) * 8;
     tile_group_begin(&bar, 0, tile_mode_, tid);
-    uint32_t staged = tile_issue<uint32_t, R5_TW, R5_TH>(s_raw, ts_input, t.input_tex, bx0 - R5_AX, by0 - 1, &bar, tile_mode_, tid, 256);
-    staged += tile_issue<float, R5_TW, R5_TH>(s_depth, ts_depth, t.depth_tex, bx0 - R5_AX, by0 - 1, &bar, tile_mode_, tid, 256);
+    uint32_t staged = tile_issue<uint32_t, R5_TW, R5_TH>(s_raw, t.input_tex, bx0 - R5_AX, by0 - 1, &bar, tile_mode_, tid, 256);
+    staged += tile_issue<float, R5_TW, R5_TH>(s_depth, t.depth_tex, bx0 - R5_AX, by0 - 1, &bar, tile_mode_, tid, 256);
     tile_group_wait(&bar, 0, tile_mode_, staged, tid);
     for (int i = tid; i < R5_LW * R5_TH; i += 256) {
         const int lx = i % R5_LW, ly = i / R5_LW;
@@ -759,9 +750,7 @@ int kjb_pass_rtr_trace(kjb_context* c, const kjb_rtr_trace_args* a) {
     IrcacheBufs ircache; if (check_ircache_bindings(c, P, a->ircache, ircache)) return 1;
     RtrTraceImgs t{img_ro(a->gbuffer_tex), img_ro(a->depth_tex), img_ro(a->rtdgi_tex), img_ro(a->sky_cube_tex), img_rw(a->out0_tex), img_rw(a->out1_tex), img_rw(a->out2_tex), img_rw(a->rng_out_tex)};
     KJB_ROWS(c, H);
-    if (ircache.bound() && c->debug_serial) KJB_LAUNCH(c, k_rtr_trace_serial, KJB_DIMS(dim3(1), dim3(32)), c->g, t, bn, F4A(a->gbuffer_tex_size), a->reuse_rtdgi_rays, ircache);
-    else if (ircache.bound()) KJB_LAUNCH_ORDERED(c, k_rtr_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, t, bn, F4A(a->gbuffer_tex_size), a->reuse_rtdgi_rays, ircache);
-    else KJB_LAUNCH(c, k_rtr_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, t, bn, F4A(a->gbuffer_tex_size), a->reuse_rtdgi_rays, ircache);
+    KJB_LAUNCH_CACHE(c, ircache.bound(), k_rtr_trace, KJB_GRID2D(W, H, KJB_RAY_BX, KJB_RAY_BY), c->g, t, bn, F4A(a->gbuffer_tex_size), a->reuse_rtdgi_rays, ircache);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_rtr_validate(kjb_context* c, const kjb_rtr_validate_args* a) {
@@ -776,9 +765,7 @@ int kjb_pass_rtr_validate(kjb_context* c, const kjb_rtr_validate_args* a) {
                       img_rw(a->refl_restir_invalidity_tex), img_rw(a->irradiance_history_tex), img_rw(a->reservoir_history_tex)};
     const int QW = int((W + 1) / 2), QH = int((H + 1) / 2);   // dispatched over half_res() of the half-res image (rtr.rs:229)
     kjb::Rows kjb__rows = c->rows_for(H); kjb__rows.y0 = kjb__rows.y0 / 2; kjb__rows.y1 = (kjb__rows.y1 + 1) / 2;   // scissor (half-res rows) -> quad rows
-    if (ircache.bound() && c->debug_serial) KJB_LAUNCH(c, k_rtr_validate_serial, KJB_DIMS(dim3(1), dim3(32)), c->g, t, F4A(a->gbuffer_tex_size), ircache, QW, QH);
-    else if (ircache.bound()) KJB_LAUNCH_ORDERED(c, k_rtr_validate, KJB_GRID2D(QW, QH, KJB_RAY_BX, KJB_RAY_BY), c->g, t, F4A(a->gbuffer_tex_size), ircache, QW, QH);
-    else KJB_LAUNCH(c, k_rtr_validate, KJB_GRID2D(QW, QH, KJB_RAY_BX, KJB_RAY_BY), c->g, t, F4A(a->gbuffer_tex_size), ircache, QW, QH);
+    KJB_LAUNCH_CACHE(c, ircache.bound(), k_rtr_validate, KJB_GRID2D(QW, QH, KJB_RAY_BX, KJB_RAY_BY), c->g, t, F4A(a->gbuffer_tex_size), ircache, QW, QH);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_rtr_restir_temporal(kjb_context* c, const kjb_rtr_restir_temporal_args* a) {
@@ -825,8 +812,7 @@ int kjb_pass_rtr_temporal(kjb_context* c, const kjb_rtr_temporal_args* a) {
     CHKE(a->gbuffer_tex, KJB_FMT_RGBA32_FLOAT, "gbuffer_tex", W, H); CHK(a->output_tex, KJB_FMT_RGBA16_FLOAT, "output_tex");
     RtrTemporalImgs t{img_ro(a->input_tex), img_ro(a->history_tex), img_ro(a->depth_tex), img_ro(a->ray_len_tex), img_ro(a->reprojection_tex), img_ro(a->refl_restir_invalidity_tex), img_ro(a->gbuffer_tex), img_rw(a->output_tex)};
     KJB_ROWS(c, H);
-    const TileSource ts_in = tile_source(c, a->input_tex, R5_TW, R5_TH), ts_depth = tile_source(c, a->depth_tex, R5_TW, R5_TH);
-    KJB_LAUNCH_SYNC(c, k_rtr_temporal, KJB_GRID2D(W, H, 32, 8), ts_in, ts_depth, tile_mode({&ts_in, &ts_depth}), c->g, t, F4A(a->output_tex_size));
+    KJB_LAUNCH_SYNC(c, k_rtr_temporal, KJB_GRID2D(W, H, 32, 8), tile_mode({&a->input_tex, &a->depth_tex}), c->g, t, F4A(a->output_tex_size));
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_rtr_cleanup(kjb_context* c, const kjb_rtr_cleanup_args* a) {

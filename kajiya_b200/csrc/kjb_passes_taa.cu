@@ -92,7 +92,7 @@ KJB_KERNEL(256) k_taa_reproject(const __grid_constant__ Globals g, Img history_t
 #define T2_LW 34   /* the logical (32+2)-wide footprint the decoded arrays hold */
 #define T2_TH 10
 KJB_DEVONLY float t2_pow8_sat(float luma_cutoff, float luma) { const float t = kjb_saturate(luma_cutoff / luma); return t == 1.0f ? 1.0f : kjb_pow(t, 8.0f); }
-KJB_KERNEL(256) k_taa_filter_input_tiled(const __grid_constant__ TileSource ts_input, const __grid_constant__ TileSource ts_depth, int use_tma, Img input_tex, Img depth_tex,
+KJB_KERNEL(256) k_taa_filter_input_tiled(int tile_mode_, Img input_tex, Img depth_tex,
                                          ImgW output_tex, ImgW dev_output_tex, W9 dw, Rows kjb_rows) {
     constexpr int P8 = tile_pitch<8>(T2_TW), P4 = tile_pitch<4>(T2_DW);
     __shared__ __align__(128) uint2 s_raw[P8 * T2_TH];
@@ -101,10 +101,10 @@ KJB_KERNEL(256) k_taa_filter_input_tiled(const __grid_constant__ TileSource ts_i
     __shared__ __align__(8) uint64_t bar;
     const int tid = int(threadIdx.y) * 32 + int(threadIdx.x);
     const int bx0 = int(blockIdx.x) * 32, by0 = kjb_rows.y0 + int(blockIdx.y) * 8 - 1;
-    tile_group_begin(&bar, 0, use_tma, tid);
-    uint32_t staged = tile_issue<uint2, T2_TW, T2_TH>(s_raw, ts_input, input_tex, bx0 - T2_AX, by0, &bar, use_tma, tid, 256);
-    staged += tile_issue<float, T2_DW, T2_TH>(s_depth, ts_depth, depth_tex, bx0 - T2_DX, by0, &bar, use_tma, tid, 256);
-    tile_group_wait(&bar, 0, use_tma, staged, tid);
+    tile_group_begin(&bar, 0, tile_mode_, tid);
+    uint32_t staged = tile_issue<uint2, T2_TW, T2_TH>(s_raw, input_tex, bx0 - T2_AX, by0, &bar, tile_mode_, tid, 256);
+    staged += tile_issue<float, T2_DW, T2_TH>(s_depth, depth_tex, bx0 - T2_DX, by0, &bar, tile_mode_, tid, 256);
+    tile_group_wait(&bar, 0, tile_mode_, staged, tid);
     for (int i = tid; i < T2_LW * T2_TH; i += 256) {
         const int lx = i % T2_LW, ly = i / T2_LW;
         const float3 c = taa_input_remap(half4_to_float4(s_raw[ly * P8 + lx + (T2_AX - 1)]));
@@ -167,16 +167,16 @@ KJB_KERNEL(256) k_taa_filter_history(Img input_tex, ImgW output_tex, float4 its,
 
 // Tiled variant for the native-resolution case (input extent == output extent, k == 1: every tap lies in the block's 34x10 footprint):
 // RGB->YCbCr once per texel, pow(1, 8) shortcut in the first pass as in T2.
-KJB_KERNEL(256) k_taa_filter_history_tiled(const __grid_constant__ TileSource ts_input, int use_tma, Img input_tex, ImgW output_tex, float4 its, float4 ots, W25t dw, Rows kjb_rows) {
+KJB_KERNEL(256) k_taa_filter_history_tiled(int tile_mode_, Img input_tex, ImgW output_tex, float4 its, float4 ots, W25t dw, Rows kjb_rows) {
     constexpr int P8 = tile_pitch<8>(T2_TW);
     __shared__ __align__(128) uint2 s_raw[P8 * T2_TH];
     __shared__ float s_y[T2_LW * T2_TH], s_cb[T2_LW * T2_TH], s_cr[T2_LW * T2_TH];
     __shared__ __align__(8) uint64_t bar;
     const int tid = int(threadIdx.y) * 32 + int(threadIdx.x);
     const int bx0 = int(blockIdx.x) * 32 - 1, by0 = kjb_rows.y0 + int(blockIdx.y) * 8 - 1;   // logical footprint origin
-    tile_group_begin(&bar, 0, use_tma, tid);
-    const uint32_t staged = tile_issue<uint2, T2_TW, T2_TH>(s_raw, ts_input, input_tex, bx0 + 1 - T2_AX, by0, &bar, use_tma, tid, 256);
-    tile_group_wait(&bar, 0, use_tma, staged, tid);
+    tile_group_begin(&bar, 0, tile_mode_, tid);
+    const uint32_t staged = tile_issue<uint2, T2_TW, T2_TH>(s_raw, input_tex, bx0 + 1 - T2_AX, by0, &bar, tile_mode_, tid, 256);
+    tile_group_wait(&bar, 0, tile_mode_, staged, tid);
     for (int i = tid; i < T2_LW * T2_TH; i += 256) {
         const int lx = i % T2_LW, ly = i / T2_LW;
         const float3 c = rgb_to_ycbcr(xyz(half4_to_float4(s_raw[ly * P8 + lx + (T2_AX - 1)])));
@@ -403,7 +403,7 @@ KJB_DEV void taa_px(const Globals& g, const TaaImgs& t, float4 its, float4 ots, 
 #define T7_HW 36
 #define T7_HH 12
 template <bool NATIVE>
-KJB_DEVONLY void taa_tiled_block(const TileSource& ts_history, const TileSource& ts_input, int use_tma, const Globals& g, const TaaImgs& t, float4 its, float4 ots, const W25t& bw, const Rows& kjb_rows) {
+KJB_DEVONLY void taa_tiled_block(int tile_mode_, const Globals& g, const TaaImgs& t, float4 its, float4 ots, const W25t& bw, const Rows& kjb_rows) {
     constexpr int PH = tile_pitch<8>(T7_HW), PI = tile_pitch<8>(T2_TW);
     __shared__ __align__(128) uint2 s_hraw[PH * T7_HH];
     __shared__ __align__(128) uint2 s_iraw[NATIVE ? PI * T2_TH : 2];
@@ -412,10 +412,10 @@ KJB_DEVONLY void taa_tiled_block(const TileSource& ts_history, const TileSource&
     __shared__ __align__(8) uint64_t bar;
     const int tid = int(threadIdx.y) * 32 + int(threadIdx.x);
     const int bx0 = int(blockIdx.x) * 32, by0 = kjb_rows.y0 + int(blockIdx.y) * 8;
-    tile_group_begin(&bar, 0, use_tma, tid);
-    uint32_t staged = tile_issue<uint2, T7_HW, T7_HH>(s_hraw, ts_history, t.history_tex, bx0 - 2, by0 - 2, &bar, use_tma, tid, 256);
-    if (NATIVE) staged += tile_issue<uint2, T2_TW, T2_TH>(s_iraw, ts_input, t.input_tex, bx0 - T2_AX, by0 - 1, &bar, use_tma, tid, 256);
-    tile_group_wait(&bar, 0, use_tma, staged, tid);
+    tile_group_begin(&bar, 0, tile_mode_, tid);
+    uint32_t staged = tile_issue<uint2, T7_HW, T7_HH>(s_hraw, t.history_tex, bx0 - 2, by0 - 2, &bar, tile_mode_, tid, 256);
+    if (NATIVE) staged += tile_issue<uint2, T2_TW, T2_TH>(s_iraw, t.input_tex, bx0 - T2_AX, by0 - 1, &bar, tile_mode_, tid, 256);
+    tile_group_wait(&bar, 0, tile_mode_, staged, tid);
     for (int i = tid; i < T7_HW * T7_HH; i += 256) s_hist[i] = half4_to_float4(s_hraw[(i / T7_HW) * PH + (i % T7_HW)]);
     if (NATIVE) for (int i = tid; i < T2_LW * T2_TH; i += 256) {
         const float3 c = taa_input_remap(half4_to_float4(s_iraw[(i / T2_LW) * PI + (i % T2_LW) + (T2_AX - 1)]));
@@ -429,11 +429,11 @@ KJB_DEVONLY void taa_tiled_block(const TileSource& ts_history, const TileSource&
     if (NATIVE) taa_px(g, t, its, ots, bw, x, y, hist, [&](int bx, int by, int dx, int dy) { const int ti = (by - by0 + 1 + dy) * T2_LW + (bx - bx0 + 1 + dx); return f3(s_y[ti], s_cb[ti], s_cr[ti]); });
     else taa_px(g, t, its, ots, bw, x, y, hist, [&](int bx, int by, int dx, int dy) { return taa_input_remap(ld_rgba16f(t.input_tex, bx + dx, by + dy)); });
 }
-KJB_KERNEL(256) k_taa_tiled(const __grid_constant__ TileSource ts_history, const __grid_constant__ TileSource ts_input, int use_tma, const __grid_constant__ Globals g, const __grid_constant__ TaaImgs t, float4 its, float4 ots, const __grid_constant__ W25t bw, Rows kjb_rows) {
-    taa_tiled_block<true>(ts_history, ts_input, use_tma, g, t, its, ots, bw, kjb_rows);
+KJB_KERNEL(256) k_taa_tiled(int tile_mode_, const __grid_constant__ Globals g, const __grid_constant__ TaaImgs t, float4 its, float4 ots, const __grid_constant__ W25t bw, Rows kjb_rows) {
+    taa_tiled_block<true>(tile_mode_, g, t, its, ots, bw, kjb_rows);
 }
-KJB_KERNEL(256) k_taa_tiled_upsampling(const __grid_constant__ TileSource ts_history, int use_tma, const __grid_constant__ Globals g, const __grid_constant__ TaaImgs t, float4 its, float4 ots, const __grid_constant__ W25t bw, Rows kjb_rows) {
-    taa_tiled_block<false>(ts_history, ts_history, use_tma, g, t, its, ots, bw, kjb_rows);
+KJB_KERNEL(256) k_taa_tiled_upsampling(int tile_mode_, const __grid_constant__ Globals g, const __grid_constant__ TaaImgs t, float4 its, float4 ots, const __grid_constant__ W25t bw, Rows kjb_rows) {
+    taa_tiled_block<false>(tile_mode_, g, t, its, ots, bw, kjb_rows);
 }
 
 #define F4A(a) f4((a)[0], (a)[1], (a)[2], (a)[3])
@@ -457,8 +457,7 @@ int kjb_pass_taa_filter_input(kjb_context* c, const kjb_taa_filter_input_args* a
     CHKE(a->dev_output_tex, KJB_FMT_RGBA16_FLOAT, "dev_output_tex", W, H);
     W9 dw; for (int y = -1; y <= 1; ++y) for (int x = -1; x <= 1; ++x) dw.w[(y + 1) * 3 + (x + 1)] = kjb_exp(-(0.8f / float(1 * 1)) * float(x * x + y * y));
     KJB_ROWS(c, H);
-    const TileSource ts_in = tile_source(c, a->input_tex, T2_TW, T2_TH), ts_depth = tile_source(c, a->depth_tex, T2_DW, T2_TH);
-    KJB_LAUNCH_SYNC(c, k_taa_filter_input_tiled, KJB_GRID2D(W, H, 32, 8), ts_in, ts_depth, tile_mode({&ts_in, &ts_depth}), img_ro(a->input_tex), img_ro(a->depth_tex), img_rw(a->output_tex), img_rw(a->dev_output_tex), dw);
+    KJB_LAUNCH_SYNC(c, k_taa_filter_input_tiled, KJB_GRID2D(W, H, 32, 8), tile_mode({&a->input_tex, &a->depth_tex}), img_ro(a->input_tex), img_ro(a->depth_tex), img_rw(a->output_tex), img_rw(a->dev_output_tex), dw);
     KJB_PASS_EPILOGUE(c, P);
 }
 int kjb_pass_taa_filter_history(kjb_context* c, const kjb_taa_filter_history_args* a) {
@@ -467,10 +466,9 @@ int kjb_pass_taa_filter_history(kjb_context* c, const kjb_taa_filter_history_arg
     const int k = (a->input_tex_size[0] / a->output_tex_size[0] > 1.75f) ? 2 : 1;
     W25t dw; for (int y = -2; y <= 2; ++y) for (int x = -2; x <= 2; ++x) dw.w[(y + 2) * 5 + (x + 2)] = kjb_exp(-(0.8f / float(k * k)) * float(x * x + y * y));
     KJB_ROWS(c, H);
-    if (k == 1 && a->input_tex.width == W && a->input_tex.height == H) {
-        const TileSource ts_in = tile_source(c, a->input_tex, T2_TW, T2_TH);
-        KJB_LAUNCH_SYNC(c, k_taa_filter_history_tiled, KJB_GRID2D(W, H, 32, 8), ts_in, tile_mode({&ts_in}), img_ro(a->input_tex), img_rw(a->output_tex), F4A(a->input_tex_size), F4A(a->output_tex_size), dw);
-    } else
+    if (k == 1 && a->input_tex.width == W && a->input_tex.height == H)
+        KJB_LAUNCH_SYNC(c, k_taa_filter_history_tiled, KJB_GRID2D(W, H, 32, 8), tile_mode({&a->input_tex}), img_ro(a->input_tex), img_rw(a->output_tex), F4A(a->input_tex_size), F4A(a->output_tex_size), dw);
+    else
         KJB_LAUNCH(c, k_taa_filter_history, KJB_GRID2D(W, H, 32, 8), img_ro(a->input_tex), img_rw(a->output_tex), F4A(a->input_tex_size), F4A(a->output_tex_size), k, dw);
     KJB_PASS_EPILOGUE(c, P);
 }
@@ -511,13 +509,10 @@ int kjb_pass_taa(kjb_context* c, const kjb_taa_args* a) {
     t.temporal_output_tex = img_rw(a->temporal_output_tex); t.output_tex = img_rw(a->output_tex); t.smooth_var_output_tex = img_rw(a->smooth_var_output_tex); t.velocity_output_tex = img_rw(a->velocity_output_tex);
     W25t bw; for (int y = -2; y <= 2; ++y) for (int x = -2; x <= 2; ++x) { const float ox = float(x) * 1.0f, oy = float(y) * 1.0f; bw.w[(y + 2) * 5 + (x + 2)] = kjb_exp(-(ox * ox + oy * oy)); }
     KJB_ROWS(c, H);
-    if (a->input_tex.width == W && a->input_tex.height == H) {
-        const TileSource ts_h = tile_source(c, a->history_tex, T7_HW, T7_HH), ts_i = tile_source(c, a->input_tex, T2_TW, T2_TH);
-        KJB_LAUNCH_SYNC(c, k_taa_tiled, KJB_GRID2D(W, H, 32, 8), ts_h, ts_i, tile_mode({&ts_h, &ts_i}), c->g, t, F4A(a->input_tex_size), F4A(a->output_tex_size), bw);
-    } else {
-        const TileSource ts_h = tile_source(c, a->history_tex, T7_HW, T7_HH);
-        KJB_LAUNCH_SYNC(c, k_taa_tiled_upsampling, KJB_GRID2D(W, H, 32, 8), ts_h, tile_mode({&ts_h}), c->g, t, F4A(a->input_tex_size), F4A(a->output_tex_size), bw);
-    }
+    if (a->input_tex.width == W && a->input_tex.height == H)
+        KJB_LAUNCH_SYNC(c, k_taa_tiled, KJB_GRID2D(W, H, 32, 8), tile_mode({&a->history_tex, &a->input_tex}), c->g, t, F4A(a->input_tex_size), F4A(a->output_tex_size), bw);
+    else
+        KJB_LAUNCH_SYNC(c, k_taa_tiled_upsampling, KJB_GRID2D(W, H, 32, 8), tile_mode({&a->history_tex}), c->g, t, F4A(a->input_tex_size), F4A(a->output_tex_size), bw);
     KJB_PASS_EPILOGUE(c, P);
 }
 

@@ -1,17 +1,13 @@
-// Screen-space tile staging for the stencil / gather kernels: one TMA bulk-tensor copy (cp.async.bulk.tensor.2d, completion on an
-// mbarrier) brings the (block + apron) footprint of an image into shared memory — the copy engine does the addressing, the bounds
-// handling (texels outside the image arrive as zeros, which is exactly the ABI's "reads outside an image return 0") and the wait costs one
-// elected thread a handful of instructions instead of every thread a guarded LDG per texel.  Warp-level exchange helpers (SHFL) live here
-// too.  Under the test-only CPU launch emulator (KJB_EMU) the same calls are plain loops / a shared scratch array.
+// Screen-space tile staging for the stencil / gather kernels: the (block + apron) footprint of an image arrives in shared memory as one
+// bulk copy per tile row (cp.async.bulk, completion on an mbarrier) — the copy engine moves the rows and the lanes of warp 0 only issue
+// them, instead of every thread a guarded LDG per texel; parts of the footprint outside the image are zero-filled, which is the ABI's
+// "reads outside an image return 0".  Warp-level exchange helpers (SHFL) live here too.  Under the test-only CPU launch emulator
+// (KJB_EMU) the same calls are plain loops / a shared scratch array.
 //
-// Tensor maps are built on the host (kjb::tile_source, kjb_api.cu) with cuTensorMapEncodeTiled fetched through
-// cudaGetDriverEntryPoint (no libcuda link).  Both TMA forms need 16-byte aligned rows: images whose row pitch is not a multiple of 16 bytes
-// (odd test extents) are staged with cooperative guarded loads instead — same contents.
+// Bulk copies need 16-byte aligned rows: images whose base or row pitch is not a multiple of 16 bytes (odd test extents) are staged
+// with cooperative guarded loads instead — same contents.  The host picks the form per launch (kjb::tile_mode, kjb_context.h).
 #pragma once
 #include "kjb_device.cuh"
-#if !defined(KJB_EMU)
-#include <cuda.h>
-#endif
 
 #if defined(KJB_EMU)
 #define KJB_DEVONLY inline
@@ -20,12 +16,6 @@
 #endif
 
 namespace kjb {
-
-#if defined(KJB_EMU)
-struct TileSource { int tensor_ok, rows_ok; };
-#else
-struct alignas(64) TileSource { CUtensorMap map; int tensor_ok, rows_ok; int pad[14]; };   // tensor_ok: `map` is encoded; rows_ok: base and row pitch are 16-byte aligned
-#endif
 
 // number of texels of a tile row as staged in shared memory: the box width rounded up so that a row is a whole number of 16-byte units
 template <int TEXEL_BYTES> constexpr int tile_pitch(int w) { return ((w * TEXEL_BYTES + 15) / 16 * 16) / TEXEL_BYTES; }
@@ -53,25 +43,19 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void bulk_load_row(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {   // 16-byte aligned on both sides, bytes % 16 == 0
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
-}
 #endif
 
 // Staging protocol (every thread of the block executes all calls, uniform control flow):
 //     tile_group_begin(bar, phase, mode, tid);                                       // first group of the block: initialises the mbarrier
-//     bytes += tile_issue<T, TW, TH>(dst, src, img, x0, y0, bar, mode, tid, nthreads);   // once per tile: TW x TH texels whose top-left texel is (x0, y0)
+//     bytes += tile_issue<T, TW, TH>(dst, img, x0, y0, bar, mode, tid, nthreads);        // once per tile: TW x TH texels whose top-left texel is (x0, y0)
 //     tile_group_wait(bar, phase, mode, bytes, tid);                                 // arms the barrier with the group's byte count and waits: tiles visible
 // `dst` has a row pitch of tile_pitch<sizeof(T)>(TW) texels and is 128-byte aligned; `phase` counts the groups this block has already pushed
 // through `bar` (0 for the first).  `mode` is one value per launch, chosen by the host (tile_mode()):
-//   KJB_TILE_TMA_TENSOR  cp.async.bulk.tensor.2d through the image's tensor map (SASS UTMALDG): any x0, the copy engine zero-fills outside the image
-//   KJB_TILE_TMA_ROWS    one cp.async.bulk per tile row issued by the lanes of warp 0 (SASS UBLKCP): x0 * sizeof(T) must be a multiple of 16;
-//                        parts of the tile outside the image are zero-filled with ordinary stores
-//   KJB_TILE_LOADS       guarded loads by every thread (rows not 16-byte aligned — odd test extents — and the CPU emulator)
+//   KJB_TILE_ROWS   one cp.async.bulk per tile row issued by the lanes of warp 0 (SASS UBLKCP): x0 * sizeof(T) must be a multiple of 16;
+//                   parts of the tile outside the image are zero-filled with ordinary stores
+//   KJB_TILE_LOADS  guarded loads by every thread (rows not 16-byte aligned — odd test extents — and the CPU emulator)
 #define KJB_TILE_LOADS 0
-#define KJB_TILE_TMA_TENSOR 1
-#define KJB_TILE_TMA_ROWS 2
+#define KJB_TILE_ROWS 1
 template <typename T, int TW, int TH> constexpr uint32_t tile_bytes() { return uint32_t(tile_pitch<int(sizeof(T))>(TW) * TH * sizeof(T)); }
 
 KJB_DEVONLY void tile_group_begin(uint64_t* bar, uint32_t phase, int mode, int tid) {
@@ -80,15 +64,10 @@ KJB_DEVONLY void tile_group_begin(uint64_t* bar, uint32_t phase, int mode, int t
 #endif
 }
 template <typename T, int TW, int TH>
-KJB_DEVONLY uint32_t tile_issue(T* dst, const TileSource& src, const Img& img, int x0, int y0, uint64_t* bar, int mode, int tid, int nthreads) {
+KJB_DEVONLY uint32_t tile_issue(T* dst, const Img& img, int x0, int y0, uint64_t* bar, int mode, int tid, int nthreads) {
     constexpr int PITCH = tile_pitch<int(sizeof(T))>(TW);
 #if !defined(KJB_EMU)
-    if (mode == KJB_TILE_TMA_TENSOR) {
-        // the map describes the image as rows of 32-bit words (4/8/16-byte texels) or of its 1/2-byte elements: scale the x coordinate
-        if (tid == 0) tma_load_2d(dst, &src.map, x0 * (sizeof(T) >= 4 ? int(sizeof(T) / 4) : 1), y0, bar);
-        return uint32_t(PITCH * TH * sizeof(T));
-    }
-    if (mode == KJB_TILE_TMA_ROWS) {
+    if (mode == KJB_TILE_ROWS) {
         const int xa = x0 < 0 ? 0 : x0, xb = x0 + PITCH < img.w ? x0 + PITCH : img.w;            // texel columns that exist
         const int ya = y0 < 0 ? 0 : y0, yb = y0 + TH < img.h ? y0 + TH : img.h;
         const bool any = xb > xa && yb > ya;
@@ -119,7 +98,7 @@ KJB_DEVONLY void tile_group_wait(uint64_t* bar, uint32_t phase, int mode, uint32
     if (mode != KJB_TILE_LOADS) {
         if (tid == 0) mbar_expect_tx(bar, bytes);     // the one arrival of the phase; copies that already landed have pre-decremented the count
         mbar_wait(bar, phase & 1u);
-        if (mode == KJB_TILE_TMA_ROWS) __syncthreads();   // border zero-fill was done with ordinary stores
+        __syncthreads();   // border zero-fill was done with ordinary stores
         return;
     }
 #endif

@@ -89,19 +89,21 @@ def test_ircache_lockstep(oracle_lib, emu_lib):
 
 def test_ircache_moving_camera_scroll_and_recycle(oracle_lib, emu_lib):
     """Cascade scrolling (scroll_cascades.hlsl), deallocation of scrolled-out cells, aging and pool recycling, through the
-    one-thread `_serial` twin kernels (kjb_set_debug_serial) on the kernel side."""
+    serial forms of the cache-touching kernels (kjb_set_debug_serial) on the kernel side — once with the cache alone, once with
+    glossy reflections on, so that the reflection trace and validate passes run their serial forms too."""
     scene, view = scenes.cornell_box()
-    kw = dict(enable_ircache=True, spatial_reuse_pass_count=1)
-    wa, wb = parity.make_world(oracle_lib, scene, 80, 48, **kw), parity.make_world(emu_lib, scene, 80, 48, **kw)
-    wb.set_debug_serial(True)
-    peak = 0
-    for f, v in enumerate(_moving_views(view, 16)):
-        wa.render_frame(**v); wb.render_frame(**v)
-        bad = parity.compare_images(wa, wb)
-        assert not bad, (f, bad[:5])
-        peak = max(peak, int(wb.image("ircache.meta_buf").ravel()[3]))
-    meta = wb.image("ircache.meta_buf").ravel()
-    assert meta[3] < peak and meta[2] > meta[3]           # entries were recycled: alloc_count fell below its peak and below entry_count
+    for sc, rtr in ((scene, False), (_glossy(scene), True)):
+        kw = dict(enable_ircache=True, enable_rtr=rtr, spatial_reuse_pass_count=1)
+        wa, wb = parity.make_world(oracle_lib, sc, 80, 48, **kw), parity.make_world(emu_lib, sc, 80, 48, **kw)
+        wb.set_debug_serial(True)
+        peak = 0
+        for f, v in enumerate(_moving_views(view, 16)):
+            wa.render_frame(**v); wb.render_frame(**v)
+            bad = parity.compare_images(wa, wb)
+            assert not bad, (rtr, f, bad[:5])
+            peak = max(peak, int(wb.image("ircache.meta_buf").ravel()[3]))
+        meta = wb.image("ircache.meta_buf").ravel()
+        assert meta[3] < peak and meta[2] > meta[3]       # entries were recycled: alloc_count fell below its peak and below entry_count
 
 
 def _glossy(scene):

@@ -1,11 +1,11 @@
-"""profiles/r02_sass_excerpts.txt: which of our kernels contain TMA-engine copies (UBLKCP = cp.async.bulk, UTMALDG = cp.async.bulk.tensor), transaction
+"""profiles/r02_sass_excerpts.txt: which of our kernels contain TMA-engine copies (UBLKCP = cp.async.bulk), transaction
 barriers (SYNCS.*) and warp shuffles (SHFL.*) — from `cuobjdump -sass` of the shipping objects (no GPU needed).   python tools/sass_excerpts.py"""
 import subprocess, re, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 objs = ['kjb_passes_taa.cu.o', 'kjb_passes_rtdgi.cu.o', 'kjb_passes_rtr.cu.o', 'kjb_passes_ircache.cu.o', 'kjb_api.cu.o']
-out = ["# SASS evidence (cuobjdump -sass of kajiya_b200/csrc/_obj/*.o, sm_90a, the shipping build): TMA-engine copies (UBLKCP = cp.async.bulk, UTMALDG = cp.async.bulk.tensor),",
+out = ["# SASS evidence (cuobjdump -sass of kajiya_b200/csrc/_obj/*.o, sm_90a, the shipping build): TMA-engine copies (UBLKCP = cp.async.bulk),",
        "# transaction barriers (SYNCS.*), warp shuffles (SHFL.*) per kernel: instruction counts and one line per distinct form.  Regenerate: python tools/sass_excerpts.py", ""]
-pat = re.compile(r'UBLKCP|UTMALDG|SYNCS\.|SHFL\.|ELECT')
+pat = re.compile(r'UBLKCP|SYNCS\.|SHFL\.|ELECT')
 for o in objs:
     txt = subprocess.run(['cuobjdump', '-sass', os.path.join(ROOT, 'kajiya_b200/csrc/_obj', o)], stdout=subprocess.PIPE, text=True).stdout
     fn, hits = None, {}
