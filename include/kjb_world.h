@@ -64,7 +64,8 @@ typedef struct kjb_world_frame {
      * geometric normal A2R10G10B10, velocity RGBA16F — i.e. what kajiya's raster pass would hand over. */
     const void *host_gbuffer, *host_depth, *host_geometric_normal, *host_velocity;
     /* Optional host destination for the frame's result (rtdgi screen irradiance, RGBA16F full-res; the TAA
-     * output RGBA16F when TAA is enabled).  Copied device->host inside the call when non-NULL. */
+     * output RGBA16F when TAA is enabled).  Copied device->host inside the call when non-NULL.  A tile-sharded
+     * world writes only its rows of it (kjb_world_result_rows). */
     void *host_result;
     /* Device-resident G-buffer ring for benchmarking with inputs already in HBM: capture_slot = k > 0 stores this frame's
      * G-buffer inputs (after the raster stand-in / upload) in ring slot k; replay_slot = k > 0 binds ring slot k as the
@@ -112,6 +113,10 @@ int  kjb_world_reset_reference_accumulation(kjb_world *w);
 /* block until every streaming frame submitted so far has delivered its host_result */
 int  kjb_world_wait(kjb_world *w);
 uint32_t kjb_world_frame_index(kjb_world *w);
+/* Rows [*y0, *y1) of the frame's result image (the TAA output, temporal_upscale_height rows; the render-res result without TAA) that this world
+ * owns: what a tile-sharded frame writes into host_result, at the same rows of a whole-frame buffer.  Band boundary b (half-res rows) maps to
+ * result row floor(RH * min(2b, render_height) / render_height), so the ranks' rows partition [0, RH) for any heights.  Untiled: [0, RH). */
+int  kjb_world_result_rows(kjb_world *w, uint32_t *y0, uint32_t *y1);
 /* Look up a live image by its reference resource name ("rtdgi.radiance:0", "gbuffer", "rtdgi.irradiance", ...). */
 int  kjb_world_get_image(kjb_world *w, const char *name, kjb_image *out);
 /* names of all live images, '\n' separated (test harness iterates them for per-pass parity) */

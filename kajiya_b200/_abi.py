@@ -104,6 +104,9 @@ class KjbLib:
             "kjb_world_render_frame": (C.c_int, [P, C.POINTER(WorldFrame)]),
             "kjb_world_render_reference": (C.c_int, [P, C.POINTER(WorldFrame), C.c_uint32]),
             "kjb_world_frame_index": (C.c_uint32, [P]),
+            "kjb_world_result_rows": (C.c_int, [P, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+            "kjb_buffer_upload": (C.c_int, [P, C.POINTER(Buffer), C.c_uint64, P, C.c_uint64]),
+            "kjb_buffer_download": (C.c_int, [P, C.POINTER(Buffer), C.c_uint64, P, C.c_uint64]),
             "kjb_world_wait": (C.c_int, [P]),
             "kjb_world_get_image": (C.c_int, [P, C.c_char_p, C.POINTER(Image)]),
             "kjb_world_image_names": (C.c_char_p, [P]),

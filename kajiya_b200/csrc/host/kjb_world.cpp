@@ -150,11 +150,18 @@ struct kjb_world {
         kjb_set_scissor(ctx, a * scale, b * scale);
     }
     void rows_all() { if (tiled) kjb_set_scissor(ctx, 0, 0); }
-    void rows_full(uint32_t e_full) {   // full-res pass: owned full-res rows grown by e_full rows
-        if (!tiled) return;
-        const uint32_t a = ty0 * 2 > e_full ? ty0 * 2 - e_full : 0, b = ty1 * 2 + e_full;
-        kjb_set_scissor(ctx, a, b);
+    void rows_span(int64_t a, int64_t b) { if (tiled) kjb_set_scissor(ctx, uint32_t(std::max<int64_t>(a, 0)), uint32_t(std::max<int64_t>(b, 1))); }   // rows [a, b) of the pass's grid
+    // The row grids of a tile-sharded frame.  A band is half-res rows [b0, b1); its rows of a full-res image are [2·b0, 2·b1) clipped to H (odd
+    // heights), and of the result image (RH rows: the TAA output, else the render-res result) the ONE ownership rule o(b) = ⌊RH·min(2b, H) / H⌋ at
+    // each band boundary.  o(0) = 0, o(HH) = RH and o is monotone, so the ranks' result rows partition [0, RH) for any RH; without upsampling
+    // o is the full-res rule.  kjb_world_result_rows reports them.
+    enum Grid : uint32_t { GRID_HALF, GRID_FULL, GRID_OUT };
+    uint32_t RH = 0;   // rows of the result image
+    uint32_t grid_row(Grid g, uint32_t b) const {
+        const uint32_t f = std::min(2 * b, H);
+        return g == GRID_HALF ? b : g == GRID_FULL ? f : uint32_t(uint64_t(RH) * f / H);
     }
+    void band_rows(Grid g, uint32_t r, uint32_t& y0, uint32_t& y1) const { uint32_t b0, b1; band(r, HH, b0, b1); y0 = grid_row(g, b0); y1 = grid_row(g, b1); }
     bool use_graph = true, graph_open = false;   // kjb_world_set_cuda_graph
     // Async compute (kjb_world_set_async_compute): the irradiance-cache chain of a frame (maintenance, cache rays, sum: ~10 small latency-bound launches)
     // runs on the async pass queue.  It needs nothing of this frame's screen-space inputs, only that the LAST frame's cache users are done, so it
@@ -233,10 +240,10 @@ int kjb_world_create(kjb_context* ctx, const kjb_world_desc* desc, kjb_world** o
     w->OW = desc->temporal_upscale_width ? desc->temporal_upscale_width : w->W; w->OH = desc->temporal_upscale_height ? desc->temporal_upscale_height : w->H;
     // Tiles + irradiance cache: every rank keeps its OWN replica of the cache, fed by the rays of its band and halos (SURVEY §8e "replicas
     // only" fall-back: the cache is one global racy structure and does not shard by rows; results stay statistically equivalent, which is all
-    // the cache promises on one GPU too).  Tiles + reflections / lit composite: not yet (rtr samples this frame's GI anywhere on screen).
+    // the cache promises on one GPU too).  Tiles + lit composite: not yet.
     if (desc->tile_count > 1 && desc->enable_lighting) { delete w; return 1; }   // the lit composite (shadow denoiser history) does not shard yet
+    w->RH = desc->enable_taa ? w->OH : w->H;
     if (desc->tile_count > 1) {
-        if (w->OW != w->W || w->OH != w->H || (w->H & 1)) { delete w; return 1; }   // tiles + temporal upscaling / odd heights: not supported
         w->tiled = true; w->trank = desc->tile_rank; w->tcount = desc->tile_count;
         w->band(w->trank, w->HH, w->ty0, w->ty1);
     }
@@ -381,6 +388,12 @@ int kjb_world_set_blue_noise(kjb_world* w, const uint8_t* rgba) {
 }
 
 uint32_t kjb_world_frame_index(kjb_world* w) { return w->frame_idx; }
+int kjb_world_result_rows(kjb_world* w, uint32_t* y0, uint32_t* y1) {
+    if (!w || !y0 || !y1) return 1;
+    if (w->tiled) w->band_rows(kjb_world::GRID_OUT, w->trank, *y0, *y1);
+    else { *y0 = 0; *y1 = w->RH; }
+    return 0;
+}
 int kjb_world_set_spatial_resolve_offsets(kjb_world* w, const int32_t* t) {
     if (!t) return 1;
     w->spatial_resolve_offsets.assign(t, t + 4 * KJB_SPATIAL_RESOLVE_OFFSET_COUNT);
@@ -524,10 +537,55 @@ static void end_frame(kjb_world* w) {
 // temporal filter 3x3, the resolve's world-space footprint is clamped to 0.1 of the screen height (resolve.hlsl:201-207) = H/40 half-res
 // rows (+ 8 % for the outermost tap + 2), the reservoir history is searched within 14 half-res px of the reprojected pixel
 // (rtr_restir_temporal.hlsl rpx_offset_radius) and validated in 2x2 quads.
-struct TileHalos { uint32_t d11, d10, d9, spatial_last, d6, d5, d4, halo, border; uint32_t r_cleanup, r_temporal, r_resolve, r_rt, r_validate, r_border; };
+//
+// TAA (taa.rs) runs on two row grids.  "reproject taa" and "taa" write the output grid (OW x OH); "taa filter input / history", "taa input prob" and
+// "taa prob filter / filter2" the input grid (the render extent).  A band owns the output rows o(b0)..o(b1) (kjb_world::grid_row), and the input-grid
+// passes run on the input rows under them, [i0, i1): output row y reads input row ry = ⌊(y + 0.5)·IH/OH⌋ as the unjittered 3x3's centre
+// (unjitter_taa.hlsl:68, k_taa_tiled*: sample_image_unjitter_taa2), for its input probability and its reprojection texel (taa.hlsl:109,
+// reproject_history.hlsl:45).  The host evaluates the kernels' float expression, so [i0, i1) is exact; with a ratio of 1 it is the full-res band.
+// Halos on the input grid, consumer first (kjb_passes_taa.cu):
+//   taa prob filter2  0   taa reads the probability at ry only;
+//   taa prob filter   5   filter2 reads a 5x5 at stride 2 (:265-266) = ±4, + 1;
+//   taa input prob    6   filter reads 3x3 (:247);
+//   taa filter history 8  input prob reads the filtered history at the nearest texel of the jittered uv (:224) = ±1, + 1;
+//   taa filter input 10   input prob reads the input deviation 3x3 at stride 2 (:220) = ±2;
+//   the GI result (TAA's input) 11 = filter input's 3x3 (:120); the unjitter's 3x3 (:284) is inside.  tile_halos' `x` = 6 half-res rows holds it,
+//   plus g = how far [i0, i1) reaches past the band's full-res rows (at most one row when upsampling), rounded up to half-res rows.
+// "reproject taa" on the output grid: "taa filter history" at input row y reads output rows ⌊(y + 0.5)/IH·OH + 1e-3⌋ ± k (:150-151, k ≤ 2), and
+// taa its 5x5 blurred history (:322-325) inside that range.  So reproject runs on the rows the filter reads from input rows [i0 - 8, i1 + 8),
+// grown by 4: k plus two rows for the truncations of the float mapping (12 output rows at a ratio of 1, as without upsampling).
+// The TAA histories (output grid) are read next frame by reproject's Catmull-Rom fetch (:62-77: rows texPos1 - 1 .. texPos1 + 2 through bilinear
+// taps = ±3) and by input prob / taa bilinearly (±1) at the reprojected uv: the exchanged border is reproject's halo + 3 + the motion bound, one
+// render row per frame = ⌈OH/H⌉ output rows (16 rows at a ratio of 1).
+struct TaaRows { int64_t o0, o1, i0, i1, rep0, rep1; };
+static TaaRows taa_rows(const kjb_world* w, uint32_t r) {
+    TaaRows t{};
+    uint32_t o0, o1; w->band_rows(kjb_world::GRID_OUT, r, o0, o1);
+    const float irs = float(w->H) / float(w->RH), inv_ih = 1.0f / float(w->H), oh = float(w->RH);
+    auto in_row = [&](int64_t y) { return int64_t(uint32_t((float(y) + 0.5f) * irs)); };                       // k_taa_tiled*, k_taa_reproject: rx, ry
+    auto out_row = [&](int64_t y) { return int64_t(std::floor((float(y) + 0.5f) * inv_ih * oh + 1e-3f)); };   // t3_filter: sy
+    t.o0 = o0; t.o1 = o1;
+    t.i0 = in_row(o0); t.i1 = o1 > o0 ? in_row(o1 - 1) + 1 : t.i0;
+    t.rep0 = out_row(t.i0 - 8) - 4; t.rep1 = out_row(t.i1 + 7) + 5;
+    return t;
+}
+// the same for every rank (the exchange layout depends on it): the largest of the bands'
+static void taa_reach(const kjb_world* w, uint32_t& g, uint32_t& border) {
+    uint32_t e = 0; g = 0;
+    for (uint32_t r = 0; r < w->tcount; ++r) {
+        const TaaRows t = taa_rows(w, r);
+        uint32_t f0, f1; w->band_rows(kjb_world::GRID_FULL, r, f0, f1);
+        g = uint32_t(std::max<int64_t>({int64_t(g), int64_t(f0) - t.i0, t.i1 - int64_t(f1)}));
+        e = uint32_t(std::max<int64_t>({int64_t(e), t.o0 - t.rep0, t.rep1 - t.o1}));
+    }
+    border = e + 3 + (w->RH + w->H - 1) / w->H;
+}
+struct TileHalos { uint32_t d11, d10, d9, spatial_last, d6, d5, d4, halo, border; uint32_t r_cleanup, r_temporal, r_resolve, r_rt, r_validate, r_border; uint32_t taa_border; };
 static TileHalos tile_halos(const kjb_world* w) {
     TileHalos h{};
-    const uint32_t x = w->desc.enable_taa ? 6u : 0u;
+    uint32_t g = 0;
+    if (w->tiled && w->desc.enable_taa) taa_reach(w, g, h.taa_border);
+    const uint32_t x = w->desc.enable_taa ? 6u + (g + 1) / 2 : 0u;
     h.r_cleanup = x; h.r_temporal = x + 13; h.r_resolve = h.r_temporal + 1; h.r_rt = h.r_resolve + w->H / 36 + 4; h.r_validate = h.r_rt + 18; h.r_border = h.r_validate + 4;
     uint32_t sum_r = 0;
     for (uint32_t i = 0; i < w->desc.spatial_reuse_pass_count; ++i) sum_r += i == 0 ? 32u : (i == 1 ? 16u : 8u);
@@ -540,7 +598,7 @@ static uint32_t spatial_radius(uint32_t pass_idx) { return pass_idx == 0 ? 32u :
 
 static const uint32_t TILE_TOP_ROWS = 16;   // half-res rows at the top of the image kept valid on every rank (pixel (0,0) dependency)
 
-struct XchgItem { kjb_image img; uint32_t scale; uint32_t border; };   // border in image rows; 0 = whole band
+struct XchgItem { kjb_image img; kjb_world::Grid grid; uint32_t border; };   // `grid`: which rows of the image a band owns; border in image rows, 0 = whole band
 
 // ONE all-gather per frame: every rank contributes the top and bottom `border` rows of its band of each temporal image (its
 // whole band for the full-res GI history, which the next frame's rays sample at arbitrary screen positions), and copies the
@@ -548,26 +606,30 @@ struct XchgItem { kjb_image img; uint32_t scale; uint32_t border; };   // border
 static int tile_exchange(kjb_world* w, const std::vector<XchgItem>& items_in, uint32_t queue, int set = 0) {
     kjb_context* ctx = w->ctx;
     const uint32_t n = w->tcount;
-    uint32_t band_max = 0, band_min = 0xffffffffu;
-    for (uint32_t r = 0; r < n; ++r) { uint32_t b0, b1; w->band(r, w->HH, b0, b1); band_max = std::max(band_max, b1 - b0); band_min = std::min(band_min, b1 - b0); }
+    // the fewest and the most rows a band owns of each item's image
+    std::vector<uint32_t> rows_min(items_in.size(), 0xffffffffu), rows_max(items_in.size(), 0);
+    for (size_t i = 0; i < items_in.size(); ++i) for (uint32_t r = 0; r < n; ++r) {
+        uint32_t y0, y1; w->band_rows(items_in[i].grid, r, y0, y1);
+        rows_min[i] = std::min(rows_min[i], y1 - y0); rows_max[i] = std::max(rows_max[i], y1 - y0);
+    }
     // One whole-band image and equal bands (this frame's GI for the reflection rays at 2 / 4 GPUs): the image IS the concatenation of the ranks' bands, so the
     // all-gather runs in place on it — no staging buffers, no pack / unpack launches.
-    if (items_in.size() == 1 && items_in[0].border == 0 && band_max == band_min && n > 1) {
+    if (items_in.size() == 1 && items_in[0].border == 0 && rows_max[0] == rows_min[0] && n > 1) {
         const kjb_image& img = items_in[0].img;
-        const uint64_t band_bytes = uint64_t(img.width) * kjb_format_texel_bytes(img.format) * band_max * items_in[0].scale;
+        const uint64_t band_bytes = uint64_t(img.width) * kjb_format_texel_bytes(img.format) * rows_max[0];
         if (band_bytes * n == uint64_t(img.width) * kjb_format_texel_bytes(img.format) * img.height)
             return kjb_allgather_on(ctx, queue, (const char*)img.data + band_bytes * w->trank, img.data, band_bytes);
     }
     // narrow bands (many ranks): when the two border strips of a band touch or overlap, send the band once instead of twice
     std::vector<XchgItem> items = items_in;
-    for (XchgItem& it : items) if (it.border && 2 * it.border >= band_min * it.scale) it.border = 0;
+    for (size_t i = 0; i < items.size(); ++i) if (items[i].border && 2 * items[i].border >= rows_min[i]) items[i].border = 0;
     // layout of one rank's contribution
     std::vector<uint64_t> off(items.size()), strip_bytes(items.size());
     uint64_t total = 0;
     for (size_t i = 0; i < items.size(); ++i) {
         const uint64_t row_bytes = uint64_t(items[i].img.width) * kjb_format_texel_bytes(items[i].img.format);
-        const uint32_t rows_max = items[i].border ? std::min(items[i].border, band_max * items[i].scale) : band_max * items[i].scale;
-        strip_bytes[i] = row_bytes * rows_max;
+        const uint32_t rows = items[i].border ? std::min(items[i].border, rows_max[i]) : rows_max[i];
+        strip_bytes[i] = row_bytes * rows;
         off[i] = total; total += strip_bytes[i] * (items[i].border ? 2 : 1);
     }
     total = (total + 255) / 256 * 256;
@@ -577,7 +639,7 @@ static int tile_exchange(kjb_world* w, const std::vector<XchgItem>& items_in, ui
         w->xchg_bytes_per_rank[set] = total;
     }
     auto strips_of = [&](uint32_t r, const XchgItem& it, uint32_t out[2][2]) {   // [strip][row0,row1) in image rows
-        uint32_t b0, b1; w->band(r, w->HH, b0, b1); b0 *= it.scale; b1 *= it.scale;
+        uint32_t b0, b1; w->band_rows(it.grid, r, b0, b1);
         if (!it.border) { out[0][0] = b0; out[0][1] = b1; out[1][0] = out[1][1] = 0; return; }
         const uint32_t k = std::min(it.border, b1 - b0);
         out[0][0] = b0; out[0][1] = b0 + k; out[1][0] = b1 - k; out[1][1] = b1;
@@ -607,7 +669,7 @@ static int tile_exchange(kjb_world* w, const std::vector<XchgItem>& items_in, ui
             // Reservoirs that never selected a sample keep payload 0 == pixel (0,0) (reservoir.hlsl:18-24), so restir_temporal /
             // restir_spatial / restir_resolve dereference the state of pixel (0,0) from anywhere on screen: the first rows of the
             // image are a global dependency and travel to every rank.
-            const uint32_t top = items[i].border ? TILE_TOP_ROWS * items[i].scale : 0;
+            const uint32_t top = items[i].border ? w->grid_row(items[i].grid, TILE_TOP_ROWS) : 0;
             const uint32_t iv[2][2] = {{need0, need1}, {0, need0 > top ? top : 0}};
             for (int k = 0; k < (items[i].border ? 2 : 1); ++k) for (int v = 0; v < 2; ++v) {
                 uint32_t a = std::max(st[k][0], iv[v][0]), b = std::min(st[k][1], iv[v][1]);
@@ -631,17 +693,21 @@ static void tile_exchange_frame(kjb_world* w) {
     kjb_context* ctx = w->ctx;
     const TileHalos th2 = tile_halos(w);
     std::vector<XchgItem> items;
-    auto add = [&](const PingPong& pp, uint32_t scale, uint32_t border) { auto it = w->images.find(pp.history_key); if (it != w->images.end()) items.push_back({it->second, scale, border}); };
-    add(w->temporal2_tex, 2, 0);
-    add(w->temporal2_variance_tex, 2, 2 * (th2.d10 + 2));
-    add(w->temporal_radiance_tex, 1, th2.border); add(w->temporal_ray_orig_tex, 1, th2.border); add(w->temporal_ray_tex, 1, th2.border);
-    add(w->temporal_reservoir_tex, 1, th2.border); add(w->temporal_candidate_tex, 1, th2.border); add(w->temporal_invalidity_tex, 1, th2.border);
-    add(w->temporal_hit_normal_tex, 1, th2.border);
-    if (w->desc.enable_taa) { add(w->taa_temporal_tex, 2, 16); add(w->taa_temporal_velocity_tex, 2, 16); add(w->taa_temporal_smooth_var_tex, 2, 16); }
+    auto add = [&](const PingPong& pp, kjb_world::Grid grid, uint32_t border) { auto it = w->images.find(pp.history_key); if (it != w->images.end()) items.push_back({it->second, grid, border}); };
+    const kjb_world::Grid HALF = kjb_world::GRID_HALF, FULL = kjb_world::GRID_FULL;
+    add(w->temporal2_tex, FULL, 0);
+    add(w->temporal2_variance_tex, FULL, 2 * (th2.d10 + 2));
+    add(w->temporal_radiance_tex, HALF, th2.border); add(w->temporal_ray_orig_tex, HALF, th2.border); add(w->temporal_ray_tex, HALF, th2.border);
+    add(w->temporal_reservoir_tex, HALF, th2.border); add(w->temporal_candidate_tex, HALF, th2.border); add(w->temporal_invalidity_tex, HALF, th2.border);
+    add(w->temporal_hit_normal_tex, HALF, th2.border);
+    if (w->desc.enable_taa) {   // output-grid histories (taa.rs:19-27)
+        add(w->taa_temporal_tex, kjb_world::GRID_OUT, th2.taa_border); add(w->taa_temporal_velocity_tex, kjb_world::GRID_OUT, th2.taa_border);
+        add(w->taa_temporal_smooth_var_tex, kjb_world::GRID_OUT, th2.taa_border);
+    }
     if (w->desc.enable_rtr) {   // what RtrRenderer reads as history next frame
-        add(w->rtr_temporal_irradiance_tex, 1, th2.r_border); add(w->rtr_temporal_ray_orig_tex, 1, th2.r_border); add(w->rtr_temporal_ray_tex, 1, th2.r_border);
-        add(w->rtr_temporal_reservoir_tex, 1, th2.r_border); add(w->rtr_temporal_rng_tex, 1, th2.r_border); add(w->rtr_temporal_hit_normal_tex, 1, th2.r_border);
-        add(w->rtr_temporal_tex, 2, 2 * (th2.r_resolve + 4)); add(w->rtr_ray_len_tex, 2, 2 * (th2.r_resolve + 4));
+        add(w->rtr_temporal_irradiance_tex, HALF, th2.r_border); add(w->rtr_temporal_ray_orig_tex, HALF, th2.r_border); add(w->rtr_temporal_ray_tex, HALF, th2.r_border);
+        add(w->rtr_temporal_reservoir_tex, HALF, th2.r_border); add(w->rtr_temporal_rng_tex, HALF, th2.r_border); add(w->rtr_temporal_hit_normal_tex, HALF, th2.r_border);
+        add(w->rtr_temporal_tex, FULL, 2 * (th2.r_resolve + 4)); add(w->rtr_ray_len_tex, FULL, 2 * (th2.r_resolve + 4));
     }
     const uint32_t queue = w->profiling ? KJB_QUEUE_COMPUTE : KJB_QUEUE_COMM;
     w->pass_begin("tile border all-gather");
@@ -977,7 +1043,7 @@ static kjb_image* rtr_render(kjb_world* w, kjb_image& gbuffer, kjb_image& depth,
     if (w->tiled && !w->err && !w->stopped) {
         // Reflection rays land anywhere on screen and read THIS frame's GI there (reflection_trace_common.inc.hlsl, USE_SCREEN_GI_REPROJECTION):
         // every rank contributes its band of the filtered GI and receives the others' — the frame's second (and last) collective.
-        std::vector<XchgItem> gi; gi.push_back({rtdgi_irradiance, 2, 0});
+        std::vector<XchgItem> gi; gi.push_back({rtdgi_irradiance, kjb_world::GRID_FULL, 0});
         w->pass_begin("tile gi all-gather");
         if (tile_exchange(w, gi, KJB_QUEUE_COMPUTE, 1)) w->err = 1;
         w->pass_end();
@@ -1068,6 +1134,7 @@ static kjb_image* rtr_render(kjb_world* w, kjb_image& gbuffer, kjb_image& depth,
 static kjb_image* taa_render(kjb_world* w, kjb_image& input_tex, kjb_image& reprojection_map, kjb_image& depth_tex) {
     kjb_context* ctx = w->ctx;
     const uint32_t OW = w->OW, OH = w->OH, IW = input_tex.width, IH = input_tex.height;
+    const TaaRows tr = taa_rows(w, w->trank);   // tile-sharded frames: the band's output / input rows (tile_halos)
     kjb_image *temporal_output_tex, *history_tex; w->get_output_and_history(w->taa_temporal_tex, OW, OH, KJB_FMT_RGBA16_FLOAT, temporal_output_tex, history_tex);
     kjb_image *temporal_velocity_output_tex, *velocity_history_tex; w->get_output_and_history(w->taa_temporal_velocity_tex, OW, OH, KJB_FMT_RG16_FLOAT, temporal_velocity_output_tex, velocity_history_tex);
     kjb_image& reprojected_history_img = w->img("taa.reprojected_history", OW, OH, KJB_FMT_RGBA16_FLOAT);
@@ -1075,36 +1142,36 @@ static kjb_image* taa_render(kjb_world* w, kjb_image& input_tex, kjb_image& repr
     {
         kjb_taa_reproject_args a{}; a.history_tex = *history_tex; a.reprojection_tex = reprojection_map; a.depth_tex = depth_tex; a.output_tex = reprojected_history_img;
         a.closest_velocity_output = closest_velocity_img; size4(a.input_tex_size, input_tex); size4(a.output_tex_size, reprojected_history_img);
-        w->rows_full(12); RUN("reproject taa", kjb_pass_taa_reproject(ctx, &a));
+        w->rows_span(tr.rep0, tr.rep1); RUN("reproject taa", kjb_pass_taa_reproject(ctx, &a));
     }
     kjb_image *smooth_var_output_tex, *smooth_var_history_tex; w->get_output_and_history(w->taa_temporal_smooth_var_tex, OW, OH, KJB_FMT_RGBA16_FLOAT, smooth_var_output_tex, smooth_var_history_tex);
     kjb_image& filtered_input_img = w->img("taa.filtered_input", IW, IH, KJB_FMT_RGBA16_FLOAT);
     kjb_image& filtered_input_deviation_img = w->img("taa.filtered_input_deviation", IW, IH, KJB_FMT_RGBA16_FLOAT);
-    { kjb_taa_filter_input_args a{input_tex, depth_tex, filtered_input_img, filtered_input_deviation_img}; w->rows_full(10); RUN("taa filter input", kjb_pass_taa_filter_input(ctx, &a)); }
+    { kjb_taa_filter_input_args a{input_tex, depth_tex, filtered_input_img, filtered_input_deviation_img}; w->rows_span(tr.i0 - 10, tr.i1 + 10); RUN("taa filter input", kjb_pass_taa_filter_input(ctx, &a)); }
     kjb_image& filtered_history_img = w->img("taa.filtered_history", IW, IH, KJB_FMT_RGBA16_FLOAT);
     {
         kjb_taa_filter_history_args a{}; a.input_tex = reprojected_history_img; a.output_tex = filtered_history_img;
         size4(a.input_tex_size, reprojected_history_img); size4(a.output_tex_size, input_tex);
-        w->rows_full(8); RUN("taa filter history", kjb_pass_taa_filter_history(ctx, &a));
+        w->rows_span(tr.i0 - 8, tr.i1 + 8); RUN("taa filter history", kjb_pass_taa_filter_history(ctx, &a));
     }
     kjb_image& input_prob_img = w->img("taa.input_prob", IW, IH, KJB_FMT_R16_FLOAT);
     {
         kjb_taa_input_prob_args a{}; a.input_tex = input_tex; a.filtered_input_tex = filtered_input_img; a.filtered_input_dev_tex = filtered_input_deviation_img;
         a.history_tex = reprojected_history_img; a.filtered_history_tex = filtered_history_img; a.reprojection_tex = reprojection_map; a.depth_tex = depth_tex;
         a.smooth_var_history_tex = *smooth_var_history_tex; a.velocity_history_tex = *velocity_history_tex; a.output_tex = input_prob_img; size4(a.input_tex_size, input_tex);
-        w->rows_full(6); RUN("taa input prob", kjb_pass_taa_input_prob(ctx, &a));
+        w->rows_span(tr.i0 - 6, tr.i1 + 6); RUN("taa input prob", kjb_pass_taa_input_prob(ctx, &a));
     }
     kjb_image& prob_filtered1_img = w->img("taa.prob_filtered1", IW, IH, KJB_FMT_R16_FLOAT);
-    { kjb_taa_prob_filter_args a{input_prob_img, prob_filtered1_img}; w->rows_full(5); RUN("taa prob filter", kjb_pass_taa_prob_filter(ctx, &a)); }
+    { kjb_taa_prob_filter_args a{input_prob_img, prob_filtered1_img}; w->rows_span(tr.i0 - 5, tr.i1 + 5); RUN("taa prob filter", kjb_pass_taa_prob_filter(ctx, &a)); }
     kjb_image& prob_filtered2_img = w->img("taa.prob_filtered2", IW, IH, KJB_FMT_R16_FLOAT);
-    { kjb_taa_prob_filter_args a{prob_filtered1_img, prob_filtered2_img}; w->rows_full(0); RUN("taa prob filter2", kjb_pass_taa_prob_filter2(ctx, &a)); }
+    { kjb_taa_prob_filter_args a{prob_filtered1_img, prob_filtered2_img}; w->rows_span(tr.i0, tr.i1); RUN("taa prob filter2", kjb_pass_taa_prob_filter2(ctx, &a)); }
     kjb_image& this_frame_output_img = w->img("taa.this_frame_out", OW, OH, KJB_FMT_RGBA16_FLOAT);
     {
         kjb_taa_args a{}; a.input_tex = input_tex; a.history_tex = reprojected_history_img; a.reprojection_tex = reprojection_map; a.closest_velocity_tex = closest_velocity_img;
         a.velocity_history_tex = *velocity_history_tex; a.depth_tex = depth_tex; a.smooth_var_history_tex = *smooth_var_history_tex; a.input_prob_tex = prob_filtered2_img;
         a.temporal_output_tex = *temporal_output_tex; a.output_tex = this_frame_output_img; a.smooth_var_output_tex = *smooth_var_output_tex; a.velocity_output_tex = *temporal_velocity_output_tex;
         size4(a.input_tex_size, input_tex); size4(a.output_tex_size, *temporal_output_tex);
-        w->rows_full(0); RUN("taa", kjb_pass_taa(ctx, &a));
+        w->rows_span(tr.o0, tr.o1); RUN("taa", kjb_pass_taa(ctx, &a));
     }
     return &this_frame_output_img;
 }
@@ -1148,13 +1215,14 @@ int kjb_world_render_frame(kjb_world* w, const kjb_world_frame* f) {
         // Tile-sharded frame with host inputs: every rank needs the WHOLE G-buffer (rays land anywhere on screen), but pushing 32 B/px through every
         // rank's PCIe link multiplies the host traffic by N.  Each rank uploads its band only and the bands travel between the GPUs over NVLink
         // (one all-gather, ~17x the bandwidth of a PCIe link): N-fold less host traffic per frame.
-        const uint32_t q = streaming ? KJB_QUEUE_UPLOAD : KJB_QUEUE_COMPUTE, r0 = w->ty0 * 2, rn = (w->ty1 - w->ty0) * 2;
+        const uint32_t q = streaming ? KJB_QUEUE_UPLOAD : KJB_QUEUE_COMPUTE, r0 = w->grid_row(kjb_world::GRID_FULL, w->ty0), rn = w->grid_row(kjb_world::GRID_FULL, w->ty1) - r0;
         int rc = streaming ? kjb_queue_wait_event(ctx, KJB_QUEUE_UPLOAD, EV_DONE) : 0;
         rc |= kjb_image_upload_rows_on(ctx, q, &gbuffer, f->host_gbuffer, r0, rn) | kjb_image_upload_rows_on(ctx, q, &depth, f->host_depth, r0, rn)
             | kjb_image_upload_rows_on(ctx, q, &geometric_normal, f->host_geometric_normal, r0, rn) | kjb_image_upload_rows_on(ctx, q, &velocity, f->host_velocity, r0, rn);
         if (streaming) rc |= kjb_event_record(ctx, EV_UP, KJB_QUEUE_UPLOAD) | kjb_queue_wait_event(ctx, KJB_QUEUE_COMPUTE, EV_UP);
         if (rc) return rc;
-        std::vector<XchgItem> in; in.push_back({gbuffer, 2, 0}); in.push_back({depth, 2, 0}); in.push_back({geometric_normal, 2, 0}); in.push_back({velocity, 2, 0});
+        const kjb_world::Grid FULL = kjb_world::GRID_FULL;
+        std::vector<XchgItem> in; in.push_back({gbuffer, FULL, 0}); in.push_back({depth, FULL, 0}); in.push_back({geometric_normal, FULL, 0}); in.push_back({velocity, FULL, 0});
         w->pass_begin("tile input all-gather");
         if (tile_exchange(w, in, KJB_QUEUE_COMPUTE, 2)) w->err = 1;
         w->pass_end();
@@ -1290,6 +1358,7 @@ int kjb_world_render_frame(kjb_world* w, const kjb_world_frame* f) {
     graph_close(w);
     if (!w->async_frame && w->desc.enable_ircache && kjb_event_record(ctx, EV_CACHE_USERS_DONE, KJB_QUEUE_COMPUTE)) w->err = 1;   // a later async frame orders its chain after this frame
     if (w->tiled && !w->exchanged_this_frame) tile_exchange_frame(w);   // with TAA its history images travel too: exchange at the end of the frame
+    uint32_t res0 = 0, res1 = 0; kjb_world_result_rows(w, &res0, &res1);   // a rank delivers its rows of the result (kjb_world_result_rows)
     if (streaming && !w->err) {
         kjb_image result{};
         if (kjb_world_get_image(w, result_name, &result) == 0) {
@@ -1297,7 +1366,7 @@ int kjb_world_render_frame(kjb_world* w, const kjb_world_frame* f) {
             int rc = kjb_queue_wait_event(ctx, KJB_QUEUE_COMPUTE, EV_DL);          // the previous download from this stage has drained
             rc |= kjb_image_copy(ctx, &stage, &result) | kjb_event_record(ctx, EV_DONE, KJB_QUEUE_COMPUTE);
             rc |= kjb_queue_wait_event(ctx, KJB_QUEUE_DOWNLOAD, EV_DONE);
-            rc |= w->tiled ? kjb_image_download_rows_on(ctx, KJB_QUEUE_DOWNLOAD, &stage, f->host_result, w->ty0 * 2, (w->ty1 - w->ty0) * 2)   // a rank delivers its band of the frame
+            rc |= w->tiled ? kjb_image_download_rows_on(ctx, KJB_QUEUE_DOWNLOAD, &stage, f->host_result, res0, res1 - res0)
                            : kjb_image_download_on(ctx, KJB_QUEUE_DOWNLOAD, &stage, f->host_result);
             rc |= kjb_event_record(ctx, EV_DL, KJB_QUEUE_DOWNLOAD);
             if (rc) w->err = rc;
@@ -1306,7 +1375,7 @@ int kjb_world_render_frame(kjb_world* w, const kjb_world_frame* f) {
     } else if (f->host_result && !w->err) {
         kjb_image result{};
         if (kjb_world_get_image(w, result_name, &result) == 0) {
-            if (w->tiled) kjb_image_download_rows_on(ctx, KJB_QUEUE_COMPUTE, &result, f->host_result, w->ty0 * 2, (w->ty1 - w->ty0) * 2);
+            if (w->tiled) kjb_image_download_rows_on(ctx, KJB_QUEUE_COMPUTE, &result, f->host_result, res0, res1 - res0);
             else kjb_image_download(ctx, &result, f->host_result);
             kjb_sync(ctx);
         }

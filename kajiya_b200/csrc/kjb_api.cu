@@ -113,7 +113,7 @@ void kjb_destroy(kjb_context* c) {
     dev_sync(c);
     dev_free(c->d_vertices); dev_free(c->d_meshes); dev_free(c->d_instances); dev_free(c->d_nodes); dev_free(c->d_tris); dev_free(c->d_tri_info);
     dev_free(c->d_node_parent); dev_free(c->d_refit_count); dev_free(c->d_slot_box); dev_free(c->d_tri_box); dev_free(c->d_bvh_scratch); dev_free(c->d_inst_prefix);
-    dev_free(c->d_tex_data); dev_free(c->d_tex_desc); dev_free(c->d_lights); dev_free(c->d_ray_counters); dev_free(c->d_prev_instances); dev_free(c->d_resolve_offsets);
+    dev_free(c->d_tex_data); dev_free(c->d_tex_desc); dev_free(c->d_lights); dev_free(c->d_ray_counters); dev_free(c->d_prev_instances); dev_free(c->d_resolve_offsets); dev_free(c->ag_scratch);
     for (auto& kv : c->ircache_scratch) { const auto& s = kv.second; dev_free(s.claim_rank); dev_free(s.claim_vertex); dev_free(s.life_pending); dev_free(s.scan); dev_free(s.claim_bits); dev_free(s.aux_prev); dev_free(s.entry_vertex); }
 #if !defined(KJB_EMU)
     if (c->pinned_staging) cudaFreeHost(c->pinned_staging);

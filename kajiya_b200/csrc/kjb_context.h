@@ -73,6 +73,7 @@ struct kjb_context {
 
     // multi-GPU transport (tile-sharded frames)
     kjb_allgather_fn ag_fn = nullptr; void* ag_user = nullptr; uint32_t rank = 0, nranks = 1; void* nccl_comm = nullptr;
+    void* ag_scratch = nullptr; uint64_t ag_scratch_bytes = 0;   // the callback transport's copy of this rank's part of an in-place gather
 
     // Row scissor for tile-sharded frames (SURVEY §8e): the next pass only computes rows [scissor_y0, scissor_y1) of ITS output
     // grid (0,0 = whole image).  Set by kjb_set_scissor, consumed (and kept) by every kjb_pass_* launch.

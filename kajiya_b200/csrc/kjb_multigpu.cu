@@ -99,15 +99,19 @@ int kjb_allgather_on(kjb_context* c, uint32_t queue, const void* send, void* rec
 #endif
     if (!c->ag_fn) return c->fail("kjb_allgather: no transport registered (kjb_comm_init_nccl / kjb_comm_set_callback)");
     if (dev_sync(c)) return c->fail("kjb_allgather: sync failed");
-#if !defined(KJB_EMU)
-    if (send == (const char*)recv + uint64_t(c->rank) * bytes) return c->fail("kjb_allgather: the callback transport of the CUDA build does not gather in place");
-#else
-    if (send == (const char*)recv + uint64_t(c->rank) * bytes) {   // in place (this rank's part already sits in `recv`): host transports get a separate copy of it
-        std::vector<uint8_t> tmp((const uint8_t*)send, (const uint8_t*)send + bytes);
-        return c->ag_fn(c->ag_user, tmp.data(), recv, bytes);
+    if (send == (const char*)recv + uint64_t(c->rank) * bytes) {   // in place (this rank's part already sits in `recv`): the transport gets a separate copy of it
+        if (c->ag_scratch_bytes < bytes) {
+            dev_free(c->ag_scratch); c->ag_scratch_bytes = 0;
+            c->ag_scratch = dev_alloc(bytes); if (!c->ag_scratch) return c->fail("kjb_allgather: out of device memory");
+            c->ag_scratch_bytes = bytes;
+        }
+        if (dev_d2d(c, c->ag_scratch, send, bytes) || dev_sync(c)) return c->fail("kjb_allgather: staging copy failed");
+        send = c->ag_scratch;
     }
-#endif
-    return c->ag_fn(c->ag_user, send, recv, bytes);
+    const int rc = c->ag_fn(c->ag_user, send, recv, bytes);
+    // the callback may have left its copies into `recv` in flight on any queue of the context (an upload from pageable memory returns early)
+    if (dev_sync(c)) return c->fail("kjb_allgather: sync failed");
+    return rc;
 }
 int kjb_allgather(kjb_context* c, const void* send, void* recv, uint64_t bytes) { return kjb_allgather_on(c, KJB_QUEUE_COMPUTE, send, recv, bytes); }
 int kjb_memcpy_d2d(kjb_context* c, void* dst, const void* src, uint64_t bytes) { c->invalidate_positions(); return dev_d2d(c, dst, src, bytes); }

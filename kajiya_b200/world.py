@@ -2,7 +2,7 @@
 add_mesh / add_instance / per-frame render, over the `kjb_world_*` C-ABI."""
 import ctypes as C
 import numpy as np
-from ._abi import Image, WorldDesc, WorldFrame, MeshDesc, MeshMaterial, TextureDesc, FMT_NUMPY, KjbError
+from ._abi import Image, Buffer, WorldDesc, WorldFrame, MeshDesc, MeshMaterial, TextureDesc, FMT_NUMPY, KjbError
 
 
 def quat_from_rotation_x(angle):
@@ -193,6 +193,25 @@ class World:
 
     def stop_after(self, label):
         self.d.kjb_world_set_stop_after(self.w, (label or "").encode())
+
+    def result_rows(self):
+        """(y0, y1): the rows of the result image (the TAA output, else the render-res result) this world renders and writes into host_result —
+        a tile-sharded world's band on the result grid, the whole image otherwise (kjb_world_result_rows)"""
+        y0, y1 = C.c_uint32(), C.c_uint32()
+        self._check(self.d.kjb_world_result_rows(self.w, C.byref(y0), C.byref(y1)))
+        return y0.value, y1.value
+
+    def device_read(self, ptr, nbytes):
+        """bytes of the context's memory at `ptr` (device memory on the CUDA build), e.g. the send buffer handed to a host all-gather callback"""
+        out = np.empty(int(nbytes), np.uint8)
+        self._check(self.d.kjb_buffer_download(self.ctx, C.byref(Buffer(ptr, nbytes)), 0, out.ctypes.data, nbytes))
+        return out
+
+    def device_write(self, ptr, host):
+        """copy the contiguous array `host` to the context's memory at `ptr` (the receive buffer of a host all-gather callback)"""
+        a = np.ascontiguousarray(host)
+        self._check(self.d.kjb_buffer_upload(self.ctx, C.byref(Buffer(ptr, a.nbytes)), 0, a.ctypes.data, a.nbytes))
+        self.sync()
 
     @property
     def frame_index(self):
