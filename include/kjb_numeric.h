@@ -49,18 +49,19 @@ KJB_HD float kjb_u2f(uint32_t u) {
 }
 
 /* ---- f32 <-> f16, round-to-nearest-even, IEEE (what DXC's f32tof16/f16tof32 and
- * R16G16B16A16_SFLOAT image stores do; pack_unpack.hlsl:90-100). NaN -> 0x7e00. ---- */
+ * R16G16B16A16_SFLOAT image stores do; pack_unpack.hlsl:90-100). Every NaN -> 0x7e00. ---- */
 KJB_HD uint32_t kjb_f32_to_f16(float f) {
 #if defined(__CUDA_ARCH__)
-    /* cvt.rn.f16.f32 is the same IEEE RN-even conversion; only NaN payloads are canonicalised here */
-    if (f != f) return ((kjb_f2u(f) >> 16) & 0x8000u) | 0x7e00u;
+    /* cvt.rn.f16.f32 is the same IEEE RN-even conversion; only NaNs are canonicalised here, sign included: the GPU's 0/0 is
+     * +NaN and x86's is -NaN, so a NaN a shader produces must not keep its sign to be stored the same on both */
+    if (f != f) return 0x7e00u;
     return (uint32_t)__half_as_ushort(__float2half_rn(f));
 #endif
     const uint32_t x = kjb_f2u(f);
     const uint32_t sign = (x >> 16) & 0x8000u;
     const uint32_t ax = x & 0x7fffffffu;
     if (ax >= 0x7f800000u) {                       /* inf / nan */
-        return sign | (ax > 0x7f800000u ? 0x7e00u : 0x7c00u);
+        return ax > 0x7f800000u ? 0x7e00u : (sign | 0x7c00u);
     }
     if (ax >= 0x477ff000u) {                       /* rounds to >= 65520 -> inf */
         return sign | 0x7c00u;

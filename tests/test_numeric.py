@@ -61,6 +61,18 @@ def test_minmax_nan_semantics(num):
     assert _call(num, "t_min", [1.0], [nan])[0] == 1.0 and _call(num, "t_min", [nan], [1.0])[0] == 1.0
 
 
+def test_f16_nan_is_canonical(num):
+    """Every f32 NaN, either sign and any payload, stores as 0x7e00: the GPU's 0/0 is +NaN and x86's is -NaN, and a NaN the
+    shaders produce (filter_history.hlsl:44 when every luma weight is 0) must be stored the same by the kernels and the oracle."""
+    rng = np.random.RandomState(9)
+    bits = np.concatenate([np.array([0x7fc00000, 0xffc00000, 0x7f800001, 0xff800001, 0x7fffffff, 0xffffffff], np.uint32),
+                           (0x7f800001 + rng.randint(0, 0x7fffff, 1000)).astype(np.uint32) | (rng.randint(0, 2, 1000).astype(np.uint32) << 31)])
+    x = bits.view(np.float32)
+    out = np.empty(x.size, np.uint32)
+    num.t_f2h(x.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p), C.c_int(x.size))
+    assert (out == 0x7e00).all()
+
+
 def test_f16_exhaustive_and_random(num):
     h = np.arange(65536, dtype=np.uint32); o = np.empty(65536, np.float32)
     num.t_h2f(h.ctypes.data_as(C.c_void_p), o.ctypes.data_as(C.c_void_p), C.c_int(65536))
