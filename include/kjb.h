@@ -257,7 +257,11 @@ int  kjb_event_synchronize(kjb_context *ctx, uint32_t event);                   
  * cache resolve their conflicts.  1 = decisions that do not depend on the order the threads run in, so the same inputs give the same
  * frames on every run (claimed cells get entries at the next cache chain, votes go to the smallest hash; kjb_ircache.cuh).  0 = the
  * reference's atomics as they land (scheduling dependent on the GPU; in launch order, like the oracle, in the emulator).  Set it before the
- * first frame with the cache: it cannot change once the ordered schedule holds pending claims. */
+ * first frame with the cache: it cannot change once the ordered schedule holds pending claims.
+ * Tile-sharded frames exchange the cache's pending requests exactly on schedule 1 (kjb_pass_ircache_export_pending), so every replica stays
+ * bit-identical to the single-GPU cache.  One buffer is left out of that equality: `reposition_proposal_count_buf`.  On schedule 1 no decision
+ * reads it (ageing resets it), and the replicas carry the largest count of any rank, which is non-zero exactly where the single cache's is.
+ * (include/kjb_ircache_share.h) */
 #define KJB_OPTION_ORDERED_CACHE_SCHEDULE 2u
 int  kjb_set_option(kjb_context *ctx, uint32_t option, uint32_t value);
 /* CUDA Graph replay of a frame's passes (the reference records one command buffer per frame, graph.rs:865-867; ~40 kernel launches here):
@@ -405,6 +409,7 @@ typedef struct kjb_ircache_share_args {
 } kjb_ircache_share_args;
 int kjb_pass_ircache_export_requests(kjb_context *ctx, const kjb_ircache_share_args *a);
 int kjb_pass_ircache_merge_requests(kjb_context *ctx, const kjb_ircache_share_args *a);
+/* The exact exchange for the ordered schedule: include/kjb_ircache_share.h. */
 
 
 /* ------------------------------------------------------------------ rtdgi (renderers/rtdgi.rs) */

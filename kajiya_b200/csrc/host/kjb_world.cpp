@@ -5,8 +5,10 @@
 //   RtdgiRenderer::{reproject,render,temporal,spatial}   crates/lib/kajiya/src/renderers/rtdgi.rs
 //   PingPongTemporalResource                    crates/lib/kajiya/src/renderers/mod.rs:73-103
 //   camera / view constants                     crates/lib/kajiya/src/camera.rs, rust-shaders-shared/src/view_constants.rs
-// It only calls the C-ABI in include/kjb.h.  No GPU, CUDA or oracle symbols are referenced directly.
+// It only calls the C-ABI in include/kjb.h (and, for tile-sharded frames with the cache, include/kjb_ircache_share.h).  No GPU, CUDA or oracle
+// symbols are referenced directly.
 #include "../../../include/kjb_world.h"
+#include "../../../include/kjb_ircache_share.h"
 #include <cmath>
 #include <algorithm>
 #include <cstring>
@@ -238,9 +240,9 @@ int kjb_world_create(kjb_context* ctx, const kjb_world_desc* desc, kjb_world** o
     w->W = desc->render_width; w->H = desc->render_height;
     w->HW = (w->W + 1) / 2; w->HH = (w->H + 1) / 2;   // ImageDesc::half_res = div_up (image.rs:140-142)
     w->OW = desc->temporal_upscale_width ? desc->temporal_upscale_width : w->W; w->OH = desc->temporal_upscale_height ? desc->temporal_upscale_height : w->H;
-    // Tiles + irradiance cache: every rank keeps its OWN replica of the cache, fed by the rays of its band and halos (SURVEY §8e "replicas
-    // only" fall-back: the cache is one global racy structure and does not shard by rows; results stay statistically equivalent, which is all
-    // the cache promises on one GPU too).  Tiles + lit composite: not yet.
+    // Tiles + irradiance cache: every rank keeps its OWN replica of the cache, fed by the rays of its band and halos, and the replicas exchange
+    // their requests after the frame's last cache user (ircache_share): exactly on the ordered schedule, so every replica stays the single-GPU
+    // cache, statistically on the reference's atomics.  Tiles + lit composite: not yet.
     if (desc->tile_count > 1 && desc->enable_lighting) { delete w; return 1; }   // the lit composite (shadow denoiser history) does not shard yet
     w->RH = desc->enable_taa ? w->OH : w->H;
     if (desc->tile_count > 1) {
@@ -727,15 +729,27 @@ static void graph_open_slot(kjb_world* w, uint32_t slot) {
     if (w->use_graph && !w->profiling && !w->tiled && w->frame_idx >= 4 && w->stop_after.empty() && !w->err && kjb_graph_select(w->ctx, slot) == 0 && kjb_graph_begin(w->ctx) == 0) w->graph_open = true;
 }
 static void graph_close(kjb_world* w) { if (w->graph_open) { w->graph_open = false; if (kjb_graph_end(w->ctx)) w->err = 1; } }
-// Tile-sharded frames: the replicas of the irradiance cache exchange what this frame's rays asked of them (kjb.h, kjb_pass_ircache_export_requests): one small
-// all-gather + one merge launch per other rank.  With async compute it runs on the async queue — right in front of the next frame's cache chain, under the
-// reflection filters and TAA of this frame.
+// Tile-sharded frames: the replicas of the irradiance cache exchange what this frame's rays asked of them (kjb.h), in one all-gather.  On the ordered
+// schedule the exchange is exact (kjb_pass_ircache_export_pending: every replica stays the single-GPU cache, bit for bit); on the reference's atomics it is
+// statistical (kjb_pass_ircache_export_requests: one small record per live entry, one merge launch per other rank).  With async compute it runs on the async
+// queue — right in front of the next frame's cache chain, under the reflection filters and TAA of this frame.
+// The CPU oracle links this driver too but renders no tile-sharded frames and has no ordered schedule: the entry points it lacks are weak references.
+extern "C" int kjb_get_option(kjb_context*, uint32_t, uint32_t*) __attribute__((weak));
+extern "C" int kjb_pass_ircache_export_pending(kjb_context*, const kjb_ircache_pending_args*) __attribute__((weak));
+extern "C" int kjb_pass_ircache_merge_pending(kjb_context*, const kjb_ircache_pending_args*) __attribute__((weak));
+static bool ircache_exact_share(kjb_world* w) {
+    uint32_t ordered = 0;
+    return kjb_get_option && kjb_pass_ircache_export_pending && kjb_pass_ircache_merge_pending &&
+           kjb_get_option(w->ctx, KJB_OPTION_ORDERED_CACHE_SCHEDULE, &ordered) == 0 && ordered == 1;
+}
 static const uint32_t EV_CACHE_SHARED = 22, CACHE_SHARE_MAX_RECORDS = 32768;
 static void ircache_share(kjb_world* w) {
     kjb_context* ctx = w->ctx;
     const uint32_t n = w->tcount;
-    const uint64_t block = (uint64_t(KJB_IRCACHE_SHARE_BLOCK_BYTES(CACHE_SHARE_MAX_RECORDS)) + 255) / 256 * 256;
+    const bool exact = ircache_exact_share(w);
+    const uint64_t block = exact ? uint64_t(KJB_IRCACHE_PENDING_BLOCK_BYTES) : (uint64_t(KJB_IRCACHE_SHARE_BLOCK_BYTES(CACHE_SHARE_MAX_RECORDS)) + 255) / 256 * 256;
     if (w->xchg_bytes_per_rank[3] != block) {
+        if (w->xchg_send[3].data) { kjb_sync(ctx); kjb_buffer_free(ctx, &w->xchg_send[3]); kjb_buffer_free(ctx, &w->xchg_recv[3]); }
         if (kjb_buffer_alloc(ctx, block, &w->xchg_send[3]) || kjb_buffer_alloc(ctx, block * n, &w->xchg_recv[3])) { w->err = 1; return; }
         w->xchg_bytes_per_rank[3] = block;
     }
@@ -743,14 +757,22 @@ static void ircache_share(kjb_world* w) {
     int rc = 0;
     if (queue == KJB_QUEUE_ASYNC) rc |= kjb_queue_wait_event(ctx, KJB_QUEUE_ASYNC, EV_CACHE_USERS_DONE) | kjb_set_pass_queue(ctx, KJB_QUEUE_ASYNC);
     w->pass_begin("tile ircache all-gather");
-    kjb_ircache_share_args a{}; a.ircache = w->frame_cache; a.max_records = CACHE_SHARE_MAX_RECORDS;
-    a.block = w->xchg_send[3];
-    rc |= kjb_pass_ircache_export_requests(ctx, &a);
-    rc |= kjb_allgather_on(ctx, queue, w->xchg_send[3].data, w->xchg_recv[3].data, block);
-    for (uint32_t r = 0; r < n && !rc; ++r) {
-        if (r == w->trank) continue;
-        a.block = kjb_buffer{(char*)w->xchg_recv[3].data + block * r, block}; a.seed = w->frame_idx * n + r;
-        rc |= kjb_pass_ircache_merge_requests(ctx, &a);
+    if (exact) {   // every rank's block, this rank's own included (merging it changes nothing), in one launch
+        kjb_ircache_pending_args a{}; a.ircache = w->frame_cache; a.blocks = w->xchg_send[3]; a.block_count = 1;
+        rc |= kjb_pass_ircache_export_pending(ctx, &a);
+        rc |= kjb_allgather_on(ctx, queue, w->xchg_send[3].data, w->xchg_recv[3].data, block);
+        a.blocks = w->xchg_recv[3]; a.block_count = n;
+        if (!rc) rc |= kjb_pass_ircache_merge_pending(ctx, &a);
+    } else {
+        kjb_ircache_share_args a{}; a.ircache = w->frame_cache; a.max_records = CACHE_SHARE_MAX_RECORDS;
+        a.block = w->xchg_send[3];
+        rc |= kjb_pass_ircache_export_requests(ctx, &a);
+        rc |= kjb_allgather_on(ctx, queue, w->xchg_send[3].data, w->xchg_recv[3].data, block);
+        for (uint32_t r = 0; r < n && !rc; ++r) {
+            if (r == w->trank) continue;
+            a.block = kjb_buffer{(char*)w->xchg_recv[3].data + block * r, block}; a.seed = w->frame_idx * n + r;
+            rc |= kjb_pass_ircache_merge_requests(ctx, &a);
+        }
     }
     w->pass_end();
     if (queue == KJB_QUEUE_ASYNC) { rc |= kjb_event_record(ctx, EV_CACHE_SHARED, KJB_QUEUE_ASYNC) | kjb_set_pass_queue(ctx, KJB_QUEUE_COMPUTE); w->cache_share_pending = true; }

@@ -3,6 +3,7 @@
 #include "kjb_ircache.cuh"
 #include "kjb_bvh_build.cuh"   // the device build's kernels, compiled in this translation unit
 #include "../../include/kjb_tlas.h"
+#include "../../include/kjb_ircache_share.h"
 #include <algorithm>
 
 using namespace kjb;
@@ -494,6 +495,12 @@ int kjb_set_option(kjb_context* c, uint32_t option, uint32_t value) {
         c->ordered_cache = value != 0; return 0;
     }
     return c->fail("kjb_set_option: unknown option");
+}
+int kjb_get_option(kjb_context* c, uint32_t option, uint32_t* value) {
+    if (!value) return c->fail("kjb_get_option: null value");
+    if (option == KJB_OPTION_HALF_RES_POSITION_CACHE) { *value = c->opt_position_cache ? 1u : 0u; return 0; }
+    if (option == KJB_OPTION_ORDERED_CACHE_SCHEDULE) { *value = c->ordered_cache && !c->debug_serial ? 1u : 0u; return 0; }
+    return c->fail("kjb_get_option: unknown option");
 }
 int kjb_set_luts(kjb_context* c, const kjb_image* fg, const kjb_image* bn) {
     if (!check_img(c, *fg, KJB_FMT_RGBA16_FLOAT, "kjb_set_luts", "brdf_fg_lut", 64, 64)) return 1;

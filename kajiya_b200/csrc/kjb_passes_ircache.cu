@@ -5,6 +5,7 @@
 // so no pass needs a host round trip.  Working set: 64 MB of per-entry reservoirs (aux) + 6 MB of grid metadata — L2-resident.
 #include "kjb_context.h"
 #include "kjb_ircache.cuh"
+#include "../../include/kjb_ircache_share.h"
 
 using namespace kjb;
 
@@ -511,6 +512,52 @@ KJB_KERNEL(256) k_ircache_merge_requests(IrcacheBufs b, const uint32_t* block, u
     }
 }
 
+// ------------------------------------------------------------------ tile-sharded frames on the ordered schedule: the exact exchange of pending requests (kjb.h)
+struct PendingBlock { uint32_t* header; float4 *proposal, *claim_vertex; uint32_t *life_pending, *vote_count, *claim_cell, *claim_rank; };
+KJB_DEV PendingBlock pending_block(uint32_t* base) {   // the layout of KJB_IRCACHE_PENDING_BLOCK_BYTES
+    PendingBlock p; p.header = base;
+    p.proposal = reinterpret_cast<float4*>(base + 64); p.claim_vertex = p.proposal + MAX_ENTRIES;
+    p.life_pending = reinterpret_cast<uint32_t*>(p.claim_vertex + MAX_ENTRIES); p.vote_count = p.life_pending + MAX_ENTRIES;
+    p.claim_cell = p.vote_count + MAX_ENTRIES; p.claim_rank = p.claim_cell + MAX_ENTRIES;
+    return p;
+}
+KJB_DEV bool f4_nonzero(float4 v) { return (kjb_f2u(v.x) | kjb_f2u(v.y) | kjb_f2u(v.z) | kjb_f2u(v.w)) != 0u; }
+// per cell (after k_ircache_det_claims and the scan of its counts, as at the chain start): the n-th claimed cell in cell order is record n, the
+// first MAX_ENTRIES of them; per entry: its pending keep-alive, vote count and vote, copied densely
+KJB_KERNEL(256) k_ircache_export_pending(IrcacheBufs b, const uint32_t* claim_bits, const uint32_t* claim_scan, uint32_t* block, Rows kjb_rows) {
+    const uint32_t cell = tid1d(); if (cell >= KJB_IRCACHE_GRID_CELLS) return;
+    const PendingBlock p = pending_block(block);
+    if (cell < MAX_ENTRIES) { p.life_pending[cell] = b.life_pending[cell]; p.vote_count[cell] = b.reposition_count[cell]; p.proposal[cell] = b.reposition_proposal[cell]; }
+    if (cell < 64) {
+        const uint32_t held = claim_scan[KJB_IRCACHE_GRID_CELLS / 32 - 1];
+        p.header[cell] = cell == 0 ? (held < MAX_ENTRIES ? held : MAX_ENTRIES) : cell == 1 ? held : 0u;
+    }
+    const uint32_t w = cell >> 5, k = cell & 31u, m = claim_bits[w];
+    if (!((m >> k) & 1u)) return;
+    const uint32_t n = (w ? claim_scan[w - 1] : 0u) + kjb_popc(m & ((1u << k) - 1u));
+    if (n >= MAX_ENTRIES) return;   // never among the union's first free_count claims (kjb.h): the chain drops it on every replica
+    p.claim_cell[n] = cell; p.claim_rank[n] = b.claim_rank[cell]; p.claim_vertex[n] = b.claim_vertex[cell];
+}
+// per (block, slot): entry `slot` of the block and its claim record `slot`, merged with the lookup's own operators — the result depends on
+// neither the order of the blocks nor that of the threads, and merging a block twice (or a replica's own block) changes nothing
+KJB_KERNEL(256) k_ircache_merge_pending(IrcacheBufs b, uint32_t* blocks, uint32_t block_count, Rows kjb_rows) {
+    const uint32_t i = tid1d(); if (i >= block_count * MAX_ENTRIES) return;
+    const uint32_t j = i % MAX_ENTRIES;
+    const PendingBlock p = pending_block(blocks + uint64_t(i / MAX_ENTRIES) * (KJB_IRCACHE_PENDING_BLOCK_BYTES / 4u));
+    const uint32_t lp = p.life_pending[j], votes = p.vote_count[j];
+    if (lp) atom_max(&b.life_pending[j], lp);
+    if (votes) atom_max(&b.reposition_count[j], votes);   // not the sum: halos and the chain's own lookups would count several times
+    const float4 v = p.proposal[j];
+    if (f4_nonzero(v)) vertex_vote(&b.reposition_proposal[j], v);
+    const uint32_t claims = p.header[0] < MAX_ENTRIES ? p.header[0] : MAX_ENTRIES;
+    if (j >= claims) return;
+    const uint32_t cell = p.claim_cell[j], rank = p.claim_rank[j];
+    if (cell >= KJB_IRCACHE_GRID_CELLS || rank == 0u || rank > IRCACHE_ENTRY_RANK_COUNT) return;   // not a record the export writes
+    atom_or(&b.grid_meta[cell * 2 + 1], IRCACHE_ENTRY_META_OCCUPIED | IRCACHE_ENTRY_META_JUST_ALLOCATED);
+    atom_max(&b.claim_rank[cell], rank);
+    vertex_vote(&b.claim_vertex[cell], p.claim_vertex[j]);
+}
+
 #define BUF(b, T, min_elems, name) if (!(b).data || (b).size_bytes < uint64_t(min_elems) * sizeof(T)) return c->fail(std::string(P) + ": buffer '" name "' is null or too small")
 #define U32P(b) ((uint32_t*)(b).data)
 #define F4P(b) ((float4*)(b).data)
@@ -666,6 +713,39 @@ int kjb_pass_ircache_merge_requests(kjb_context* c, const kjb_ircache_share_args
     NO_SCISSOR;
     IrcacheBufs b = ircache_bufs(a->ircache); ircache_attach_parallel(c, b);
     KJB_LAUNCH_ORDERED(c, k_ircache_merge_requests, DIMS1D(a->max_records, 256), b, (const uint32_t*)a->block.data, a->max_records, a->seed);
+    KJB_PASS_EPILOGUE(c, P);
+}
+
+static int check_pending_args(kjb_context* c, const char* P, const kjb_ircache_pending_args* a, IrcacheBufs& b, kjb_context::IrcacheScratch& s) {
+    if (!share_bindings_ok(a->ircache)) return c->fail(std::string(P) + ": the irradiance cache is not bound");
+    BUF(a->ircache.grid_meta_buf, uint2, KJB_IRCACHE_GRID_CELLS, "grid_meta_buf"); BUF(a->ircache.life_buf, uint32_t, MAX_ENTRIES, "life_buf");
+    BUF(a->ircache.reposition_proposal_buf, float4, MAX_ENTRIES, "reposition_proposal_buf"); BUF(a->ircache.reposition_proposal_count_buf, uint32_t, MAX_ENTRIES, "reposition_proposal_count_buf");
+    if (!ircache_parallel_scratch(c, a->ircache.life_buf.data, s))
+        return c->fail(std::string(P) + ": needs the ordered cache schedule (KJB_OPTION_ORDERED_CACHE_SCHEDULE = 1, kjb_set_debug_serial off); "
+                       "the reference's atomics race, so only kjb_pass_ircache_export_requests / _merge_requests apply there");
+    if (a->block_count == 0 || a->block_count > 4096u) return c->fail(std::string(P) + ": block_count must be 1..4096");
+    if (!a->blocks.data || a->blocks.size_bytes < uint64_t(KJB_IRCACHE_PENDING_BLOCK_BYTES) * a->block_count)
+        return c->fail(std::string(P) + ": buffer 'blocks' is null or smaller than block_count * KJB_IRCACHE_PENDING_BLOCK_BYTES");
+    if (reinterpret_cast<uintptr_t>(a->blocks.data) & 15u) return c->fail(std::string(P) + ": buffer 'blocks' must be 16-byte aligned");
+    b = ircache_bufs(a->ircache); ircache_attach_parallel(c, b);
+    return 0;
+}
+int kjb_pass_ircache_export_pending(kjb_context* c, const kjb_ircache_pending_args* a) {
+    const char* P = "tile ircache export pending";
+    IrcacheBufs b; kjb_context::IrcacheScratch s; if (check_pending_args(c, P, a, b, s)) return 1;
+    if (a->block_count != 1) return c->fail(std::string(P) + ": exports exactly one block (block_count 1)");
+    NO_SCISSOR;
+    uint32_t* claim_scan = (uint32_t*)s.scan + MAX_ENTRIES;   // the chain start's own claim scan: it recomputes it before it reads it
+    KJB_LAUNCH(c, k_ircache_det_claims, DIMS1D(KJB_IRCACHE_GRID_CELLS / 32, 256), (const uint32_t*)s.claim_rank, (uint32_t*)s.claim_bits, claim_scan);
+    KJB_LAUNCH_SYNC(c, k_inclusive_prefix_scan, KJB_DIMS(dim3(1), dim3(1024)), claim_scan, KJB_IRCACHE_GRID_CELLS / 32);
+    KJB_LAUNCH(c, k_ircache_export_pending, DIMS1D(KJB_IRCACHE_GRID_CELLS, 256), b, (const uint32_t*)s.claim_bits, (const uint32_t*)claim_scan, U32P(a->blocks));
+    KJB_PASS_EPILOGUE(c, P);
+}
+int kjb_pass_ircache_merge_pending(kjb_context* c, const kjb_ircache_pending_args* a) {
+    const char* P = "tile ircache merge pending";
+    IrcacheBufs b; kjb_context::IrcacheScratch s; if (check_pending_args(c, P, a, b, s)) return 1;
+    NO_SCISSOR;
+    KJB_LAUNCH(c, k_ircache_merge_pending, DIMS1D(uint64_t(a->block_count) * MAX_ENTRIES, 256), b, U32P(a->blocks), a->block_count);
     KJB_PASS_EPILOGUE(c, P);
 }
 

@@ -6,7 +6,8 @@
 Every N = 1, 2, 4, ... up to the launched rank count is timed in turn (ranks [0, N) render, the others wait; each group gets its own NCCL
 communicator).  Prints one JSON line per N on rank 0: ms/frame (device timer events around K frames on every rank, after a barrier; the frame's G-buffer
 replayed from HBM as bench.py does), the GPU name and its power limit, and for N > 1 each rank's parity: its result rows against the same rows
-of an untiled render on the same GPU (statistical: every rank keeps a replica of the irradiance cache, DESIGN §7).  bench.py's configs[4] adds
+of an untiled render on the same GPU (bit-identical on the ordered cache schedule, the GPU's default: the ranks' cache replicas exchange their
+pending requests exactly, DESIGN §7).  bench.py's configs[4] adds
 SSAO and the lit composite, which do not shard."""
 import argparse, ctypes as C, json, os, subprocess, sys
 import numpy as np
