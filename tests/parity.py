@@ -15,6 +15,15 @@ def make_world(lib, scene, width, height, **kw):
     return w
 
 
+def glossy(scene):
+    """the Cornell box with glossy walls, so that the reflection passes really trace (roughness <= 0.6)"""
+    import copy
+    s = copy.deepcopy(scene)
+    for i, m in enumerate(s[0][0]["materials"]):
+        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
+    return s
+
+
 def world_triangles(scene):
     """gid-ordered (instance-major, as scenes.populate adds them) world-space triangles float32[n, 9] and tri_info uint32[n, 2], with the
     library's xform_point: ((m0 x + m1 y) + m2 z) + m3 in float32, no contraction"""

@@ -3,6 +3,7 @@ the CPU builds), instanced + moving geometry."""
 import ctypes as C
 import numpy as np, pytest
 import parity
+from parity import glossy
 from kajiya_b200 import scenes
 from kajiya_b200.world import World
 from kajiya_b200._abi import Image, KjbError, FMT
@@ -184,21 +185,13 @@ def test_sun_size_multiplier_at_run_time(oracle_lib, emu_lib):
         wb.set_sun_size_multiplier(-1.0)
 
 
-def _glossy_cornell(scene):
-    import copy
-    s = copy.deepcopy(scene)
-    for i, m in enumerate(s[0][0]["materials"]):
-        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
-    return s
-
-
 def test_world_renderer_knobs(oracle_lib, emu_lib):
     """sun_color_multiplier / sky_ambient (re-bake the sky cubes), RenderOverrides (closest-hit shader), debug_shading_mode (lit composite):
     each change takes effect and stays bit-exact between oracle and emulator"""
     import parity
     scene, view = scenes.cornell_box()
     kw = dict(enable_lighting=True, enable_rtr=True)
-    wa, wb = parity.make_world(oracle_lib, _glossy_cornell(scene), 64, 40, **kw), parity.make_world(emu_lib, _glossy_cornell(scene), 64, 40, **kw)
+    wa, wb = parity.make_world(oracle_lib, glossy(scene), 64, 40, **kw), parity.make_world(emu_lib, glossy(scene), 64, 40, **kw)
     def frames(n):
         for _ in range(n):
             wa.render_frame(**view); wb.render_frame(**view)

@@ -2,6 +2,7 @@
 (tests/emu) against the oracle, frame by frame, every image bit-for-bit.  (The real CUDA build is checked by test_gpu_parity.py.)"""
 import numpy as np
 import parity
+from parity import glossy
 from kajiya_b200 import scenes
 
 
@@ -92,7 +93,7 @@ def test_ircache_moving_camera_scroll_and_recycle(oracle_lib, emu_lib):
     serial forms of the cache-touching kernels (kjb_set_debug_serial) on the kernel side — once with the cache alone, once with
     glossy reflections on, so that the reflection trace and validate passes run their serial forms too."""
     scene, view = scenes.cornell_box()
-    for sc, rtr in ((scene, False), (_glossy(scene), True)):
+    for sc, rtr in ((scene, False), (glossy(scene), True)):
         kw = dict(enable_ircache=True, enable_rtr=rtr, spatial_reuse_pass_count=1)
         wa, wb = parity.make_world(oracle_lib, sc, 80, 48, **kw), parity.make_world(emu_lib, sc, 80, 48, **kw)
         wb.set_debug_serial(True)
@@ -106,20 +107,12 @@ def test_ircache_moving_camera_scroll_and_recycle(oracle_lib, emu_lib):
         assert meta[3] < peak and meta[2] > meta[3]       # entries were recycled: alloc_count fell below its peak and below entry_count
 
 
-def _glossy(scene):
-    import copy
-    s = copy.deepcopy(scene)
-    for i, m in enumerate(s[0][0]["materials"]):
-        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
-    return s
-
-
 def test_rtr_lockstep(oracle_lib, emu_lib):
     """Reflections (rtr.rs): trace (only below roughness 0.6, else the diffuse candidates are reused), validate, temporal ReSTIR,
     resolve, temporal filter, cleanup — with glossy Cornell materials so that every branch runs, camera in motion so the
     reprojection search does too."""
     scene, view = scenes.cornell_box()
-    scene = _glossy(scene)
+    scene = glossy(scene)
     kw = dict(enable_rtr=True, spatial_reuse_pass_count=1)
     wa, wb = parity.make_world(oracle_lib, scene, 88, 56, **kw), parity.make_world(emu_lib, scene, 88, 56, **kw)
     cp = np.array(view["camera_position"], np.float32)
@@ -139,7 +132,7 @@ def test_rtr_lockstep(oracle_lib, emu_lib):
 def test_rtr_with_ircache_and_taa(oracle_lib, emu_lib):
     """BASELINE config 3/4 shape: rtdgi + ircache + rtr (+ taa), every image and cache buffer bit for bit (serial cache schedule)."""
     scene, view = scenes.cornell_box()
-    _, wb, report = parity.run_lockstep(oracle_lib, emu_lib, _glossy(scene), view, 80, 48, 6, enable_rtr=True, enable_ircache=True, enable_taa=True)
+    _, wb, report = parity.run_lockstep(oracle_lib, emu_lib, glossy(scene), view, 80, 48, 6, enable_rtr=True, enable_ircache=True, enable_taa=True)
     _clean(report)
     assert wb.image("ircache.meta_buf").ravel()[3] > 50
 
@@ -201,7 +194,7 @@ def test_lighting_composite_feeds_taa(oracle_lib, emu_lib):
     whose output is what TAA then consumes; full path around it."""
     scene, view = scenes.cornell_box()
     kw = dict(enable_lighting=True, enable_rtr=True, enable_ircache=True, enable_taa=True, enable_ssao=True)
-    wa, wb, report = parity.run_lockstep(oracle_lib, emu_lib, _glossy(scene), view, 96, 60, 5, **kw)
+    wa, wb, report = parity.run_lockstep(oracle_lib, emu_lib, glossy(scene), view, 96, 60, 5, **kw)
     _clean(report)
     out = wb.image("debug_out").astype(np.float32); gi = wb.image("rtdgi.spatial_filtered").astype(np.float32)
     depth = wb.image("depth")[..., 0]
@@ -251,7 +244,7 @@ def _cornell_with_ceiling_light(lib, w, h, **kw):
     from kajiya_b200.world import World
     scene, view = scenes.cornell_box()
     world = World(lib, w, h, **kw)
-    mesh, transforms = _glossy(scene)[0]
+    mesh, transforms = glossy(scene)[0]
     hm = world.add_mesh(mesh)
     for t in transforms: world.add_instance(hm, t)
     P = np.array([[-0.3, 1.9, -0.3], [0.3, 1.9, -0.3], [0.3, 1.9, 0.3], [-0.3, 1.9, 0.3]], np.float32)

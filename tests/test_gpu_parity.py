@@ -2,6 +2,7 @@
 Bar: bit-exact for every image, integer AND float (the numeric contract pins the transcendentals; no FMA contraction)."""
 import numpy as np, pytest
 import parity
+from parity import glossy
 from kajiya_b200 import scenes
 
 pytestmark = pytest.mark.gpu
@@ -141,18 +142,10 @@ def test_ircache_parallel_statistical(oracle_lib, cuda_lib):
     assert np.sqrt(((ia - ib) ** 2).mean()) <= 0.05 * max(ia.mean(), 1e-6) + 0.05, np.sqrt(((ia - ib) ** 2).mean())
 
 
-def _glossy(scene):
-    import copy
-    s = copy.deepcopy(scene)
-    for i, m in enumerate(s[0][0]["materials"]):
-        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
-    return s
-
-
 def test_rtr_lockstep(oracle_lib, cuda_lib):
     """Reflections R1-R6 on glossy Cornell, camera in motion: every image bit for bit."""
     scene, view = scenes.cornell_box()
-    scene = _glossy(scene)
+    scene = glossy(scene)
     kw = dict(enable_rtr=True)
     wa, wb = parity.make_world(oracle_lib, scene, 160, 90, **kw), parity.make_world(cuda_lib, scene, 160, 90, **kw)
     cp = np.array(view["camera_position"], np.float32)
@@ -168,7 +161,7 @@ def test_full_pipeline_serial_schedule_bit_exact(oracle_lib, cuda_lib):
     """rtdgi + ircache + rtr + taa with the cache passes on the serial schedule: everything bit for bit on the real GPU."""
     scene, view = scenes.cornell_box()
     kw = dict(enable_rtr=True, enable_ircache=True, enable_taa=True)
-    wa, wb = parity.make_world(oracle_lib, _glossy(scene), 80, 48, **kw), parity.make_world(cuda_lib, _glossy(scene), 80, 48, **kw)
+    wa, wb = parity.make_world(oracle_lib, glossy(scene), 80, 48, **kw), parity.make_world(cuda_lib, glossy(scene), 80, 48, **kw)
     wb.set_debug_serial(True)
     for f in range(6):
         wa.render_frame(**view); wb.render_frame(**view)
@@ -353,7 +346,7 @@ def test_cuda_graph_frames_match_directly_launched_frames(cuda_lib):
     and also through the streaming host-buffer call."""
     scene, view = scenes.cornell_box()
     kw = dict(enable_rtr=True, enable_ircache=False, enable_taa=True)
-    wa, wb = parity.make_world(cuda_lib, _glossy(scene), 320, 180, **kw), parity.make_world(cuda_lib, _glossy(scene), 320, 180, **kw)
+    wa, wb = parity.make_world(cuda_lib, glossy(scene), 320, 180, **kw), parity.make_world(cuda_lib, glossy(scene), 320, 180, **kw)
     wb.set_cuda_graph(False)
     cp = np.array(view["camera_position"], np.float32)
     for f in range(12):

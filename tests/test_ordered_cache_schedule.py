@@ -9,7 +9,8 @@ import pytest
 import parity
 from kajiya_b200 import scenes
 from kajiya_b200._abi import KjbError
-from test_emu_parity import _glossy, _moving_views, _ordered_cache_invariants
+from parity import glossy
+from test_emu_parity import _moving_views, _ordered_cache_invariants
 from test_edge_cases import _cache_bindings
 
 ORDERED_CACHE_SCHEDULE = 2            # KJB_OPTION_ORDERED_CACHE_SCHEDULE (kjb.h)
@@ -124,7 +125,7 @@ def test_ordered_schedule_is_independent_of_launch_order(emu_lib, launch_order):
     and cache buffer after every frame"""
     scene, view = scenes.cornell_box()
     views = list(_moving_views(view, 16))
-    runs = _render_in_orders(emu_lib, launch_order, _glossy(scene), 80, 48, views, 1, **FULL_PATH)
+    runs = _render_in_orders(emu_lib, launch_order, glossy(scene), 80, 48, views, 1, **FULL_PATH)
     assert _first_difference(runs) is None, _first_difference(runs)
     names = set(runs[ORDERS[0]][-1])
     assert {"ircache." + b for b in CACHE_BUFFERS} <= names and {"rtr.resolved", "taa.this_frame_out"} <= names
@@ -140,7 +141,7 @@ def test_reference_atomics_depend_on_launch_order(emu_lib, launch_order):
     """control for the two tests above: with the reference's atomics (which thread claims first decides the entry) reversing the launch order
     changes the cache buffers within the first frames, so the knob does reach the cache kernels"""
     scene, view = scenes.cornell_box()
-    runs = _render_in_orders(emu_lib, launch_order, _glossy(scene), 80, 48, list(_moving_views(view, 3)), 0, orders=ORDERS[:2], **FULL_PATH)
+    runs = _render_in_orders(emu_lib, launch_order, glossy(scene), 80, 48, list(_moving_views(view, 3)), 0, orders=ORDERS[:2], **FULL_PATH)
     diff = _first_difference(runs)
     assert diff is not None and any(n in diff[2] for n in ("ircache.entry_cell_buf", "ircache.grid_meta_buf", "ircache.grid_meta_buf2")), diff
 
@@ -151,7 +152,7 @@ def test_ordered_entry_assignment_rule(emu_lib, launch_order, moving):
     claimed cell in ascending cell order takes the n-th free entry in ascending entry order; the bookkeeping invariants hold every frame"""
     scene, view = scenes.cornell_box()
     launch_order(2, 7)
-    w = parity.make_world(emu_lib, _glossy(scene), 80, 48, **FULL_PATH)
+    w = parity.make_world(emu_lib, glossy(scene), 80, 48, **FULL_PATH)
     w.set_option(ORDERED_CACHE_SCHEDULE, 1)
     views = list(_moving_views(view, 12)) if moving else [view] * 8
     checked = 0
@@ -351,7 +352,7 @@ def _gpu_against_emulator(cuda_lib, emu_lib, scene, width, height, views, **kw):
 @pytest.mark.gpu
 def test_gpu_ordered_schedule_matches_the_emulator_cornell(cuda_lib, emu_lib):
     scene, view = scenes.cornell_box()
-    _gpu_against_emulator(cuda_lib, emu_lib, _glossy(scene), 160, 90, list(_moving_views(view, 16)), **FULL_PATH)
+    _gpu_against_emulator(cuda_lib, emu_lib, glossy(scene), 160, 90, list(_moving_views(view, 16)), **FULL_PATH)
 
 
 @pytest.mark.gpu
@@ -375,7 +376,7 @@ def test_cuda_graph_frames_with_the_cache_match_directly_launched_frames(cuda_li
     buffer bit for bit against launching the kernels one by one, full path with the cache, camera in motion"""
     scene, view = scenes.cornell_box()
     kw = dict(enable_rtr=True, enable_ircache=True, enable_taa=True)
-    wa, wb = parity.make_world(cuda_lib, _glossy(scene), 320, 180, **kw), parity.make_world(cuda_lib, _glossy(scene), 320, 180, **kw)
+    wa, wb = parity.make_world(cuda_lib, glossy(scene), 320, 180, **kw), parity.make_world(cuda_lib, glossy(scene), 320, 180, **kw)
     for w in (wa, wb):
         w.set_async_compute(False)
     wb.set_cuda_graph(False)

@@ -11,24 +11,15 @@ f16 subnormals, 6e4, negative channels and neighbourhoods whose luma is all nega
 Also: a scissored run equals the unscissored run on its rows and leaves the other rows alone, and the H100 equals the oracle
 bit for bit on every synthetic case.
 """
-import copy
-import ctypes as C
 import numpy as np
 import pytest
 
 import taa_reference as ref
-from kajiya_b200._abi import Image, FMT
-
-F16, SNORM, DEPTH, RG16, R16 = FMT["RGBA16_FLOAT"], FMT["RGBA16_SNORM"], FMT["R32_FLOAT"], FMT["RG16_FLOAT"], FMT["R16_FLOAT"]
-NP = {F16: (np.float16, 4), SNORM: (np.int16, 4), DEPTH: (np.float32, 1), RG16: (np.float16, 2), R16: (np.float16, 1)}
+from pass_harness import F16, SNORM, DEPTH, RG16, R16, Runners, extent4, frame_constants
+from parity import glossy
 
 
-# ---------------------------------------------------------------- the C-ABI harness
-def _args(images, floats=0):
-    fields = [(n, Image) for n in images] + [(f"f{i}", C.c_float * 4) for i in range(floats)]
-    return type("Args", (C.Structure,), {"_fields_": fields})
-
-
+# ---------------------------------------------------------------- the passes, in the shape the C-ABI harness drives them
 PASSES = {   # entry point, image bindings in kjb.h order, float4 constants
     "reproject": ("kjb_pass_taa_reproject", ["history_tex", "reprojection_tex", "depth_tex", "output_tex", "closest_velocity_output"], 2),
     "filter_input": ("kjb_pass_taa_filter_input", ["input_tex", "depth_tex", "output_tex", "dev_output_tex"], 0),
@@ -47,110 +38,9 @@ OUTPUTS = {"reproject": ("output_tex", "closest_velocity_output"), "filter_input
            "prob_filter2": ("output_tex",), "taa": ("temporal_output_tex", "output_tex", "smooth_var_output_tex", "velocity_output_tex")}
 
 
-def frame_constants(pre_exposure_delta=1.0, delta_time_seconds=1.0 / 60.0, sample_offset_pixels=(0.0, 0.0)):
-    """kjb_frame_constants (1216 bytes, kjb.h) zero but for the three fields the TAA shaders read."""
-    fc = np.zeros(1216 // 4, np.float32)
-    fc[176:178] = sample_offset_pixels      # view_constants.sample_offset_pixels: after 11 mat4
-    fc[185] = delta_time_seconds            # after sun_direction[4], frame_index
-    fc[198] = pre_exposure_delta            # after ..., sky_ambient[4], pre_exposure, pre_exposure_prev
-    return fc
-
-
-def extent4(w, h):
-    return [float(w), float(h), float(np.float32(1) / np.float32(w)), float(np.float32(1) / np.float32(h))]
-
-
-class Runner:
-    """One context of one backend; runs one pass on host arrays and returns its outputs as raw host arrays."""
-
-    def __init__(self, lib):
-        self.lib, d = lib, lib.dll
-        self.ctx = C.c_void_p()
-        assert d.kjb_create(0 if lib.backend.startswith("cuda") else -1, C.byref(self.ctx)) == 0
-        d.kjb_set_frame_constants.restype = C.c_int
-        d.kjb_set_frame_constants.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
-        d.kjb_set_scissor.restype = C.c_int
-        d.kjb_set_scissor.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
-        for name, _, _ in PASSES.values():
-            getattr(d, name).restype = C.c_int
-            getattr(d, name).argtypes = [C.c_void_p, C.c_void_p]
-
-    def err(self):
-        return self.lib.dll.kjb_last_error(self.ctx).decode()
-
-    def close(self):
-        self.lib.dll.kjb_destroy(self.ctx)
-
-    def run(self, pass_name, inputs, outputs, consts=(), fc=None, scissor=None, sentinel=None):
-        """inputs: {binding: raw array (H, W, C) of the format's numpy type, format}; outputs: {binding: (w, h, format)}."""
-        d, ctx = self.lib.dll, self.ctx
-        entry, bindings, nf = PASSES[pass_name]
-        fc = frame_constants() if fc is None else fc
-        assert d.kjb_set_frame_constants(ctx, fc.ctypes.data, None, 0) == 0, self.err()
-        imgs, keep = {}, []
-        try:
-            for b, (arr, fmt) in inputs.items():
-                img = Image()
-                assert d.kjb_image_alloc(ctx, arr.shape[1], arr.shape[0], 1, fmt, C.byref(img)) == 0, self.err()
-                imgs[b] = img
-                arr = np.ascontiguousarray(arr)
-                keep.append(arr)
-                assert d.kjb_image_upload(ctx, C.byref(img), arr.ctypes.data) == 0, self.err()
-            for b, (w, h, fmt) in outputs.items():
-                img = Image()
-                assert d.kjb_image_alloc(ctx, w, h, 1, fmt, C.byref(img)) == 0, self.err()
-                imgs[b] = img
-                if sentinel is not None:
-                    dt, c = NP[fmt]
-                    fill = np.full(h * w * c * np.dtype(dt).itemsize, sentinel, np.uint8)
-                    keep.append(fill)
-                    assert d.kjb_image_upload(ctx, C.byref(img), fill.ctypes.data) == 0, self.err()
-            args = _args(bindings, nf)()
-            for b in bindings:
-                setattr(args, b, imgs.get(b, Image()))
-            for i, c4 in enumerate(consts):
-                getattr(args, f"f{i}")[:] = c4
-            try:
-                if scissor is not None:
-                    assert d.kjb_set_scissor(ctx, *scissor) == 0, self.err()
-                assert getattr(d, entry)(ctx, C.byref(args)) == 0, self.err()
-            finally:
-                if scissor is not None:
-                    d.kjb_set_scissor(ctx, 0, 0)
-            got = {}
-            for b, (w, h, fmt) in outputs.items():
-                dt, c = NP[fmt]
-                out = np.empty((h, w, c), dt)
-                assert d.kjb_image_download(ctx, C.byref(imgs[b]), out.ctypes.data) == 0, self.err()
-                got[b] = out
-            assert d.kjb_sync(ctx) == 0, self.err()
-            return got
-        finally:
-            d.kjb_sync(ctx)   # the uploads read `keep` and the downloads write `got` until the stream drains
-            for img in imgs.values():
-                d.kjb_image_free(ctx, C.byref(img))
-
-
-class Runners:
-    """One Runner per backend, created on first use and destroyed with the module's tests."""
-
-    def __init__(self):
-        self._by_path = {}
-
-    def __call__(self, lib):
-        if lib.path not in self._by_path:
-            self._by_path[lib.path] = Runner(lib)
-        return self._by_path[lib.path]
-
-    def close(self):
-        for r in self._by_path.values():
-            r.close()
-        self._by_path.clear()
-
-
 @pytest.fixture(scope="module")
 def runners():
-    rs = Runners()
+    rs = Runners(PASSES)
     yield rs
     rs.close()
 
@@ -522,13 +412,6 @@ def test_row_bands_gpu(gpu_runner, case):
 
 
 # ---------------------------------------------------------------- the realistic leg: the inputs a rendered frame's TAA read
-def _glossy(scene):
-    scene = copy.deepcopy(scene)
-    for i, m in enumerate(scene[0][0]["materials"]):
-        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
-    return scene
-
-
 def _halton_offset(frame_idx):
     """the frame driver's jitter: Halton(2, 3) - 0.5 of (frame_idx % 128) + 1, in float32 (world_renderer.rs:425-428)"""
     def radical_inverse(n, base):
@@ -552,7 +435,7 @@ def realistic_passes(lib):
     import parity
     from kajiya_b200 import scenes
     scene, view = scenes.cornell_box()
-    w = parity.make_world(lib, _glossy(scene), REAL_W, REAL_H, enable_taa=True, enable_rtr=True, spatial_reuse_pass_count=2,
+    w = parity.make_world(lib, glossy(scene), REAL_W, REAL_H, enable_taa=True, enable_rtr=True, spatial_reuse_pass_count=2,
                           upscale=(REAL_OW, REAL_OH))
     try:
         for f in range(REAL_FRAMES):

@@ -13,7 +13,8 @@ import torch.distributed as dist, torch.multiprocessing as mp
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, HERE)
-from test_tile_upscaled import _compare_bands, _free_port, _gloo_allgather, _glossy, _names, _view   # noqa: E402
+from parity import glossy   # noqa: E402
+from test_tile_upscaled import _compare_bands, _free_port, _gloo_allgather, _names, _view   # noqa: E402
 
 ORDERED_CACHE_SCHEDULE = 2     # KJB_OPTION_ORDERED_CACHE_SCHEDULE (kjb.h)
 MAX_ENTRIES, GRID_CELLS = 1 << 16, 32 * 32 * 32 * 12
@@ -96,7 +97,7 @@ def _worker(rank, world_size, port, cfg, ret):
     OH = up[1] if up else H
     scene, view = scenes.cornell_box()
     if rtr:
-        scene = _glossy(scene)
+        scene = glossy(scene)
     kw = dict(enable_ircache=True, enable_taa=taa, enable_rtr=rtr, spatial_reuse_pass_count=cfg.get("spatial", 1), upscale=up)
     tiled = parity.make_world(lib, scene, W, H, tile=(rank, world_size), **kw)
     calls = [0]

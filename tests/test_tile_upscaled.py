@@ -5,7 +5,7 @@ kjb_world_result_rows reports: floor(OH·min(2b, H)/H) at each band boundary.  E
 grid the image lives on, must equal the same rows of a single-process render bit for bit.  CPU: the kernel emulator with gloo
 ranks.  GPU: several rank processes on one H100 over the callback transport with host-staged gloo, and NCCL where there are
 two GPUs or more."""
-import ctypes as C, copy, os, socket, sys
+import ctypes as C, os, socket, sys
 import numpy as np, pytest
 import torch, torch.distributed as dist, torch.multiprocessing as mp
 
@@ -16,14 +16,6 @@ FRAMES = 5
 
 def _free_port():
     s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _glossy(scene):
-    """glossy walls so that the reflection passes really trace (roughness <= 0.6)"""
-    scene = copy.deepcopy(scene)
-    for i, m in enumerate(scene[0][0]["materials"]):
-        m["roughness"] = [0.05, 0.2, 0.35, 0.5, 0.8][i % 5]; m["metallic"] = [1.0, 0.0, 0.5][i % 3]
-    return scene
 
 
 def _view(view, frame, move):
@@ -101,7 +93,7 @@ def _worker(rank, world_size, port, cfg, ret):
     OH = up[1] if up else H
     scene, view = scenes.cornell_box()
     if rtr:
-        scene = _glossy(scene)
+        scene = parity.glossy(scene)
     kw = dict(enable_taa=True, spatial_reuse_pass_count=2, enable_rtr=rtr, upscale=up)
     tiled = parity.make_world(lib, scene, W, H, tile=(rank, world_size), **kw)
     calls = [0]
@@ -252,7 +244,7 @@ def _gpu_worker(rank, world_size, port, transport, W, H, up, ret):
     import parity
     lib = kajiya_b200.lib()
     scene, view = scenes.cornell_box()
-    scene = _glossy(scene)
+    scene = parity.glossy(scene)
     kw = dict(enable_taa=True, enable_rtr=True, spatial_reuse_pass_count=2, upscale=up)
     tiled = parity.make_world(lib, scene, W, H, device=device, tile=(rank, world_size), **kw)
     calls = [0]
